@@ -930,14 +930,14 @@ typedef struct SvtB200EngineStats {
     uint64_t me_pictures, dlf_frames, cdef_frames, lr_frames;
     uint64_t me_plane_uploads, me_plane_hits; /* ME plane residency cache: pictures uploaded / found resident */
     uint64_t h2d_bytes, d2h_bytes, pinned_bytes;
-    /* wall time summed over calling threads: waiting for a slot, page-locking host buffers, waiting for another
-     * thread's upload of a shared reference, issuing copies + launches, waiting for the GPU, copying results out */
-    uint64_t ns_slot_wait, ns_pin, ns_plane_wait, ns_issue, ns_sync, ns_host_copy, pin_calls;
+    /* wall time summed over calling threads: waiting for a slot, waiting for another thread's upload of a shared
+     * reference, issuing copies + launches, waiting for the GPU, copying between host pictures and pinned staging */
+    uint64_t ns_slot_wait, ns_plane_wait, ns_issue, ns_sync, ns_host_copy;
 } SvtB200EngineStats;
 
 /* device: CUDA ordinal (the integration reads SVT_CUDA_DEVICE).  Fails (no CPU fallback) when it does not exist.
- * Host buffers handed to the engine are page-locked on first use (SVT_B200_PIN_HOST=0 disables) and released in
- * svt_b200_engine_destroy, which must therefore run before the caller frees them (svt_av1_enc_deinit hook). */
+ * The engine copies host pictures through its own pinned staging: the caller's buffers stay pageable, and the engine
+ * reads or writes them only during a call. */
 SVT_B200_API int svt_b200_engine_create(int device, SvtB200Engine **out);
 SVT_B200_API void svt_b200_engine_destroy(SvtB200Engine *e);
 SVT_B200_API int svt_b200_engine_get_stats(SvtB200Engine *e, SvtB200EngineStats *out);
@@ -987,29 +987,14 @@ typedef struct SvtB200HostLrLines {
 SVT_B200_API int svt_b200_engine_lr_frame(SvtB200Engine *e, const SvtB200LrFrameParams *p, const int32_t n_units[3],
                                           const SvtB200Frame *frame, const SvtB200HostLrLines lines[3]);
 
-/* The CDEF stage of cdef_kernel (EbCdefProcess.c:510-534) for one HOST picture: strength search of every 64x64 filter
- * block -> `mse` (host, [2][nfb][64], = pcs->mse_seg) -> `decide(user, mse, apply, fb_strength_idx)` on the calling
- * thread, where the integration runs the reference's finish_cdef_search (EbEncCdef.c:1167) and fills the frame
- * strengths (damping, y/uv strength tables) and mbmi.cdef_strength per filter block (preset to -1) -> frame apply,
- * written back into `recon` (host) in place.  decide returns 1 to apply, 0 to skip the apply (the reference skips it for
- * non-reference pictures without recon output), < 0 on error.  The reconstruction stays on the device between the
- * search and the apply. */
-typedef int (*SvtB200CdefDecideFn)(void *user, const uint64_t *mse, SvtB200CdefApplyParams *apply, int8_t *fb_strength_idx);
-SVT_B200_API int svt_b200_engine_cdef_frame(SvtB200Engine *e, const SvtB200CdefSearchParams *sp, const SvtB200Frame *recon,
-                                            const SvtB200Frame *source, const uint8_t *skip8, int32_t skip_stride,
-                                            uint64_t *mse, SvtB200CdefDecideFn decide, void *user);
-/* The same preceded by the deblocking of the picture (dlf != NULL; mi: host array [mi_rows][mi_cols]): the reconstruction
- * is uploaded ONCE, deblocked on the device and handed to the CDEF stages there - for pictures whose deblocked version
- * nobody needs on the host (no loop restoration: svt_av1_loop_restoration_save_boundary_lines would read it).  When
- * `decide` returns 0 (no apply) the host reconstruction is left as it was: the reference does not filter a picture nobody
- * reads. */
-SVT_B200_API int svt_b200_engine_dlf_cdef_frame(SvtB200Engine *e, const SvtB200DlfParams *dlf, const SvtB200DlfMi *mi,
-                                                const SvtB200CdefSearchParams *sp, const SvtB200Frame *recon,
-                                                const SvtB200Frame *source, const uint8_t *skip8, int32_t skip_stride,
-                                                uint64_t *mse, SvtB200CdefDecideFn decide, void *user);
-/* The same with the strength decision on the device (svt_b200_cdef_decide instead of the callback): one upload, deblocking
- * (dlf / mi may be NULL), CDEF search, decision, CDEF apply (apply != 0), one download, ONE synchronisation.  decision /
- * fb_strength_idx: HOST outputs (frame header fields and mbmi.cdef_strength per filter block, -1 = all-skip block). */
+/* The CDEF stage of cdef_kernel (EbCdefProcess.c:510-534) for one HOST picture, preceded by the deblocking of the
+ * picture when dlf != NULL (mi: host array [mi_rows][mi_cols]): the reconstruction is uploaded ONCE, deblocked on the
+ * device and handed to the CDEF stages there - for pictures whose deblocked version nobody needs on the host (no loop
+ * restoration: svt_av1_loop_restoration_save_boundary_lines would read it).  Strength search of every 64x64 filter
+ * block, the strength decision (svt_b200_cdef_decide: finish_cdef_search, EbEncCdef.c:1167), frame apply written back
+ * into `recon` (host) in place when apply != 0, one download, ONE synchronisation.  With apply = 0 the host
+ * reconstruction is left as it was: the reference does not filter a picture nobody reads.  decision / fb_strength_idx:
+ * HOST outputs (frame header fields and mbmi.cdef_strength per filter block, -1 = all-skip block). */
 SVT_B200_API int svt_b200_engine_dlf_cdef_frame_dev(SvtB200Engine *e, const SvtB200DlfParams *dlf, const SvtB200DlfMi *mi,
                                                     const SvtB200CdefSearchParams *sp, const SvtB200CdefDecideParams *dp,
                                                     int32_t damping, int32_t apply, const SvtB200Frame *recon,

@@ -11,7 +11,6 @@
  *   SVT_CUDA=1            turn the CUDA backend on (default: off -> the build behaves exactly like the reference)
  *   SVT_CUDA_DEVICE=n     CUDA ordinal (default 0)
  *   SVT_CUDA_ME / SVT_CUDA_DLF / SVT_CUDA_CDEF / SVT_CUDA_LR = 0 to leave one stage on the CPU (default 1 when SVT_CUDA=1)
- *   SVT_CUDA_FUSE=0       deblock in the DLF stage's own GPU call instead of deferring it into the CDEF stage's call
  *   SVT_CUDA_ME_DS=1      derive the 1/4 and 1/16 ME planes on the device instead of uploading the host's
  *   SVT_CUDA_PROFILE=1    print per-stage wall time / call counts at deinit (also for the CPU path, for comparison)
  * There is NO CPU fallback once a stage is on: a failing GPU call prints the library's message and aborts.
@@ -47,11 +46,11 @@ static volatile long long g_tf_calls = 0;
 #include "svt_cuda_tf_shim.h"
 static void (*g_tf_saved[2])(void);
 
-static int            g_on = -1, g_me = 0, g_dlf = 0, g_cdef = 0, g_lr = 0, g_fuse = 0, g_me_ds = 0, g_prof = 0, g_tf = 0, g_pa = 0, g_ois = 0, g_cdef_dev = 1;
+static int            g_on = -1, g_me = 0, g_dlf = 0, g_cdef = 0, g_lr = 0, g_me_ds = 0, g_prof = 0, g_tf = 0, g_pa = 0, g_ois = 0;
 static volatile long long g_pa_calls = 0, g_ois_calls = 0;
 /* SVT_CUDA_PROFILE: host-side pieces of the deblocking / CDEF hooks (thread-ns): mode-info flattening, skip8 map, the
- * reference's finish_cdef_search inside the engine's callback, the engine call as a whole */
-static volatile long long g_ns_flatten = 0, g_ns_skip8 = 0, g_ns_decide = 0, g_ns_engine_cdef = 0;
+ * engine call as a whole */
+static volatile long long g_ns_flatten = 0, g_ns_skip8 = 0, g_ns_engine_cdef = 0;
 #define PROF_ADD(var, t_start) do { if (g_prof) __sync_fetch_and_add(&(var), now_ns() - (t_start)); } while (0)
 static SvtB200Engine *g_engine = NULL;
 static int            g_users  = 0;
@@ -94,9 +93,7 @@ void svt_cuda_backend_init(void) {
             g_dlf   = env_flag("SVT_CUDA_DLF", 1);
             g_cdef  = env_flag("SVT_CUDA_CDEF", 1);
             g_lr    = env_flag("SVT_CUDA_LR", 1);
-            g_fuse  = env_flag("SVT_CUDA_FUSE", 1);
             g_me_ds = env_flag("SVT_CUDA_ME_DS", 0);
-            g_cdef_dev = env_flag("SVT_CUDA_CDEF_DECIDE", 1); /* 0: finish_cdef_search on the host (engine callback) */
             /* parity switches, off by default: bit-exact, but per-block / per-picture round trips that do not pay */
             g_tf = env_flag("SVT_CUDA_TF", 0);
             g_pa = env_flag("SVT_CUDA_PA", 0);
@@ -119,7 +116,7 @@ void svt_cuda_backend_init(void) {
     }
 }
 
-/* svt_av1_enc_deinit hook (before the encoder frees its picture buffers: the engine page-locked them) */
+/* svt_av1_enc_deinit hook: prints the profile and releases the engine */
 void svt_cuda_backend_deinit(void) {
     if (g_prof) {
         for (int gpu = 0; gpu < 2; gpu++)
@@ -144,8 +141,8 @@ void svt_cuda_backend_deinit(void) {
                     st.ns_slot_wait / 1e6, st.ns_issue / 1e6, st.ns_plane_wait / 1e6, st.ns_sync / 1e6, st.ns_host_copy / 1e6);
         }
         if (g_prof)
-            fprintf(stderr, "SVT [CUDA profile]: host side of the filter hooks, thread-ms: flatten mode info %.1f, skip8 map %.1f, finish_cdef_search %.1f, CDEF engine calls %.1f\n",
-                    g_ns_flatten / 1e6, g_ns_skip8 / 1e6, g_ns_decide / 1e6, g_ns_engine_cdef / 1e6);
+            fprintf(stderr, "SVT [CUDA profile]: host side of the filter hooks, thread-ms: flatten mode info %.1f, skip8 map %.1f, CDEF engine calls %.1f\n",
+                    g_ns_flatten / 1e6, g_ns_skip8 / 1e6, g_ns_engine_cdef / 1e6);
         if (g_prof && (g_tf || g_pa || g_ois))
             fprintf(stderr, "SVT [CUDA profile]: tf blocks on the GPU %lld, picture-analysis pictures on the GPU %lld, open-loop intra pictures on the GPU %lld\n",
                     (long long)g_tf_calls, (long long)g_pa_calls, (long long)g_ois_calls);
@@ -415,7 +412,7 @@ static EbPictureBufferDesc *recon_of(PictureControlSet *pcs_ptr, int is_16bit) {
 
 static __thread const PictureControlSet *t_filtered = NULL; /* svt_cuda_dlf_pick_frame already deblocked this picture */
 
-/* Deblocking deferred into the CDEF stage's GPU call (svt_b200_engine_dlf_cdef_frame): the DLF stage only derives the
+/* Deblocking deferred into the CDEF stage's GPU call (svt_b200_engine_dlf_cdef_frame_dev): the DLF stage only derives the
  * parameters; the reconstruction is then uploaded once for both filters.  Only when nobody needs the deblocked picture on the
  * host: no loop restoration (its boundary lines are saved from the deblocked host picture in dlf_kernel), no statistics. */
 #include <pthread.h>
@@ -431,7 +428,7 @@ static PendingDlf      g_pend[N_PENDING];
 static pthread_mutex_t g_pend_mu = PTHREAD_MUTEX_INITIALIZER;
 
 static int fuse_ok(PictureControlSet *pcs_ptr, SequenceControlSet *scs_ptr) {
-    return g_fuse && svt_cuda_cdef_applies(pcs_ptr, scs_ptr) && scs_ptr->seq_header.cdef_level && pcs_ptr->parent_pcs_ptr->cdef_level &&
+    return svt_cuda_cdef_applies(pcs_ptr, scs_ptr) && scs_ptr->seq_header.cdef_level && pcs_ptr->parent_pcs_ptr->cdef_level &&
         !scs_ptr->seq_header.enable_restoration && !scs_ptr->static_config.stat_report;
 }
 static PendingDlf *pending_take(const PictureControlSet *pcs_ptr, int create) {
@@ -562,57 +559,8 @@ int svt_cuda_dlf_pick_frame(PictureControlSet *pcs_ptr, SequenceControlSet *scs_
  * CDEF: cdef_seg_search[16bit] of every segment + finish_cdef_search + svt_av1_cdef_frame / av1_cdef_frame16bit
  * (cdef_kernel, EbCdefProcess.c:510-534) for one picture
  * ================================================================================================================= */
-typedef struct CdefDecide {
-    PictureControlSet * pcs;
-    SequenceControlSet *scs;
-    int                 nvfb, nhfb;
-    const uint8_t *     skip8; /* [ceil(mi_rows/2)][skip_stride] */
-    int                 skip_stride, rows8, cols8;
-} CdefDecide;
-
-void finish_cdef_search(EncDecContext *context_ptr, PictureControlSet *pcs_ptr, int32_t selected_strength_cnt[64]);
-
-static int cdef_decide(void *user, const uint64_t *mse, SvtB200CdefApplyParams *ap, int8_t *fb_strength_idx) {
-    CdefDecide *             d    = (CdefDecide *)user;
-    PictureControlSet *      pcs  = d->pcs;
-    PictureParentControlSet *ppcs = pcs->parent_pcs_ptr;
-    FrameHeader *            fh   = &ppcs->frm_hdr;
-    const int                nfb  = d->nvfb * d->nhfb;
-    /* pcs->mse_seg[plane][fb][64] is what cdef_seg_search fills */
-    memcpy(pcs->mse_seg[0], mse, sizeof(uint64_t) * (size_t)nfb * TOTAL_STRENGTHS);
-    memcpy(pcs->mse_seg[1], mse + (size_t)nfb * TOTAL_STRENGTHS, sizeof(uint64_t) * (size_t)nfb * TOTAL_STRENGTHS);
-    int32_t selected_strength_cnt[64] = {0};
-    const int64_t td0 = g_prof ? now_ns() : 0;
-    finish_cdef_search(0, pcs, selected_strength_cnt);
-    PROF_ADD(g_ns_decide, td0);
-    if (!(d->scs->seq_header.enable_restoration != 0 || ppcs->is_used_as_reference_flag || d->scs->static_config.recon_enabled))
-        return 0; /* EbCdefProcess.c:527-529: the frame is not filtered when nobody reads it */
-    ap->damping = fh->cdef_params.cdef_damping;
-    for (int i = 0; i < 8; i++) {
-        ap->y_strength[i]  = fh->cdef_params.cdef_y_strength[i];
-        ap->uv_strength[i] = fh->cdef_params.cdef_uv_strength[i];
-    }
-    const Av1Common *cm = ppcs->av1_cm;
-    for (int fbr = 0; fbr < d->nvfb; fbr++)
-        for (int fbc = 0; fbc < d->nhfb; fbc++) {
-            const ModeInfo *mi = pcs->mi_grid_base[MI_SIZE_64X64 * fbr * cm->mi_stride + MI_SIZE_64X64 * fbc];
-            /* svt_sb_all_skip == every 8x8 of the filter block is skip (the map the search used) */
-            int all_skip = 1;
-            for (int r8 = 8 * fbr; r8 < AOMMIN(8 * fbr + 8, d->rows8) && all_skip; r8++)
-                for (int c8 = 8 * fbc; c8 < AOMMIN(8 * fbc + 8, d->cols8); c8++)
-                    if (!d->skip8[(size_t)r8 * d->skip_stride + c8]) {
-                        all_skip = 0;
-                        break;
-                    }
-            fb_strength_idx[fbr * d->nhfb + fbc] = (!mi || all_skip) ? -1 : mi->mbmi.cdef_strength;
-        }
-    return 1;
-}
-
 static __thread uint8_t * t_skip     = NULL;
 static __thread size_t    t_skip_cap = 0;
-static __thread uint64_t *t_mse      = NULL;
-static __thread size_t    t_mse_cap  = 0;
 
 /* Runs the whole CDEF stage of the picture (search of every filter block, finish_cdef_search, frame apply); called by
  * the thread that completes the last CDEF segment, in place of finish_cdef_search + svt_av1_cdef_frame (only when
@@ -641,13 +589,7 @@ void svt_cuda_cdef_picture(PictureControlSet *pcs_ptr, SequenceControlSet *scs_p
         t_skip     = (uint8_t *)malloc(b_skip);
         t_skip_cap = b_skip;
     }
-    const size_t n_mse = (size_t)2 * nvfb * nhfb * TOTAL_STRENGTHS;
-    if (t_mse_cap < n_mse) {
-        free(t_mse);
-        t_mse     = (uint64_t *)malloc(n_mse * sizeof(uint64_t));
-        t_mse_cap = n_mse;
-    }
-    if (!t_skip || !t_mse) die("malloc", -1);
+    if (!t_skip) die("malloc", -1);
     const int64_t ts0 = g_prof ? now_ns() : 0;
     memset(t_skip, 1, b_skip);
     ModeInfo **grid = pcs_ptr->mi_grid_base;
@@ -700,55 +642,45 @@ void svt_cuda_cdef_picture(PictureControlSet *pcs_ptr, SequenceControlSet *scs_p
     recon.height = source.height = mi_rows * 4;
     recon.bit_depth = source.bit_depth = is_16bit ? 10 : 8;
 
-    CdefDecide  d    = {pcs_ptr, scs_ptr, nvfb, nhfb, t_skip, skip_stride, rows8, (mi_cols + 1) / 2};
     PendingDlf *pend = pending_take(pcs_ptr, 0); /* deblocking deferred by the DLF stage: same upload, deblock, then CDEF */
     const int64_t te0 = g_prof ? now_ns() : 0;
-    int           rc;
-    if (g_cdef_dev && scs_ptr->seq_header.sb_size != BLOCK_128X128) {
-        /* finish_cdef_search on the device (svt_b200_cdef_decide): the picture makes one round trip.  Inputs the reference
-         * derives on the host: the picture's lambda (EbEncCdef.c:1209) and the strength table of the pick method */
-        SvtB200CdefDecideParams dp;
-        memset(&dp, 0, sizeof(dp));
-        svt_b200_cdef_decide_table(pick_method, &dp);
-        dp.mi_rows = mi_rows;
-        dp.mi_cols = mi_cols;
-        uint32_t fast_lambda = 0, full_lambda = 0;
-        (*av1_lambda_assignment_function_table[ppcs->pred_structure])(pcs_ptr, &fast_lambda, &full_lambda,
-                                                                     (uint8_t)ppcs->enhanced_picture_ptr->bit_depth,
-                                                                     (uint16_t)(uint8_t)ppcs->frm_hdr.quantization_params.base_q_idx, EB_FALSE);
-        dp.lambda = full_lambda;
-        const int apply = scs_ptr->seq_header.enable_restoration != 0 || ppcs->is_used_as_reference_flag || scs_ptr->static_config.recon_enabled;
-        SvtB200CdefDecision dec;
-        int8_t *            fb_idx = (int8_t *)malloc((size_t)nvfb * nhfb);
-        if (!fb_idx) die("malloc", -1);
-        rc = svt_b200_engine_dlf_cdef_frame_dev(g_engine, pend ? &pend->p : NULL, pend ? pend->mi : NULL, &sp, &dp, sp.pri_damping, apply,
+    /* finish_cdef_search on the device (svt_b200_cdef_decide): the picture makes one round trip.  Inputs the reference
+     * derives on the host: the picture's lambda (EbEncCdef.c:1209) and the strength table of the pick method */
+    SvtB200CdefDecideParams dp;
+    memset(&dp, 0, sizeof(dp));
+    svt_b200_cdef_decide_table(pick_method, &dp);
+    dp.mi_rows = mi_rows;
+    dp.mi_cols = mi_cols;
+    uint32_t fast_lambda = 0, full_lambda = 0;
+    (*av1_lambda_assignment_function_table[ppcs->pred_structure])(pcs_ptr, &fast_lambda, &full_lambda,
+                                                                 (uint8_t)ppcs->enhanced_picture_ptr->bit_depth,
+                                                                 (uint16_t)(uint8_t)ppcs->frm_hdr.quantization_params.base_q_idx, EB_FALSE);
+    dp.lambda = full_lambda;
+    /* EbCdefProcess.c:527-529: the frame is not filtered when nobody reads it */
+    const int apply = scs_ptr->seq_header.enable_restoration != 0 || ppcs->is_used_as_reference_flag || scs_ptr->static_config.recon_enabled;
+    SvtB200CdefDecision dec;
+    int8_t *            fb_idx = (int8_t *)malloc((size_t)nvfb * nhfb);
+    if (!fb_idx) die("malloc", -1);
+    int rc = svt_b200_engine_dlf_cdef_frame_dev(g_engine, pend ? &pend->p : NULL, pend ? pend->mi : NULL, &sp, &dp, sp.pri_damping, apply,
                                                 &recon, &source, t_skip, skip_stride, &dec, fb_idx);
-        PROF_ADD(g_ns_engine_cdef, te0);
-        if (pend) pending_release(pend);
-        if (rc) die("svt_b200_engine_dlf_cdef_frame_dev", rc);
-        /* what finish_cdef_search leaves behind (EbEncCdef.c:1276-1336) */
-        FrameHeader *fh            = &ppcs->frm_hdr;
-        fh->cdef_params.cdef_bits  = (uint8_t)dec.cdef_bits;
-        ppcs->nb_cdef_strengths    = dec.nb_cdef_strengths;
-        for (int j = 0; j < dec.nb_cdef_strengths; j++) {
-            fh->cdef_params.cdef_y_strength[j]  = dec.y_strength[j];
-            fh->cdef_params.cdef_uv_strength[j] = dec.uv_strength[j];
-        }
-        fh->cdef_params.cdef_damping = sp.pri_damping;
-        for (int fbr = 0; fbr < nvfb; fbr++)
-            for (int fbc = 0; fbc < nhfb; fbc++) {
-                const int8_t v = fb_idx[fbr * nhfb + fbc];
-                if (v >= 0) pcs_ptr->mi_grid_base[MI_SIZE_64X64 * fbr * pcs_ptr->mi_stride + MI_SIZE_64X64 * fbc]->mbmi.cdef_strength = v;
-            }
-        free(fb_idx);
-        if (g_prof) stat_add(1, ST_CDEF, t0);
-        return;
-    }
-    rc = svt_b200_engine_dlf_cdef_frame(g_engine, pend ? &pend->p : NULL, pend ? pend->mi : NULL, &sp, &recon, &source, t_skip,
-                                        skip_stride, t_mse, cdef_decide, &d);
     PROF_ADD(g_ns_engine_cdef, te0);
     if (pend) pending_release(pend);
-    if (rc) die("svt_b200_engine_dlf_cdef_frame", rc);
+    if (rc) die("svt_b200_engine_dlf_cdef_frame_dev", rc);
+    /* what finish_cdef_search leaves behind (EbEncCdef.c:1276-1336) */
+    FrameHeader *fh            = &ppcs->frm_hdr;
+    fh->cdef_params.cdef_bits  = (uint8_t)dec.cdef_bits;
+    ppcs->nb_cdef_strengths    = dec.nb_cdef_strengths;
+    for (int j = 0; j < dec.nb_cdef_strengths; j++) {
+        fh->cdef_params.cdef_y_strength[j]  = dec.y_strength[j];
+        fh->cdef_params.cdef_uv_strength[j] = dec.uv_strength[j];
+    }
+    fh->cdef_params.cdef_damping = sp.pri_damping;
+    for (int fbr = 0; fbr < nvfb; fbr++)
+        for (int fbc = 0; fbc < nhfb; fbc++) {
+            const int8_t v = fb_idx[fbr * nhfb + fbc];
+            if (v >= 0) pcs_ptr->mi_grid_base[MI_SIZE_64X64 * fbr * pcs_ptr->mi_stride + MI_SIZE_64X64 * fbc]->mbmi.cdef_strength = v;
+        }
+    free(fb_idx);
     if (g_prof) stat_add(1, ST_CDEF, t0);
 }
 

@@ -430,7 +430,7 @@ static int dlf_frame_impl(const SvtB200DlfParams *p, const SvtB200Frame *frame, 
     // the block-edge kernels move 4-sample words: planes whose base / stride are 4-sample aligned (every EbPictureBufferDesc
     // and every engine picture); other layouts take the line-per-thread kernel
     const size_t wbytes = hbd ? 8 : 4;
-    const bool aligned = !getenv("SVT_B200_DLF_LINE_KERNEL") && ((uintptr_t)frame->y % wbytes) == 0 && ((uintptr_t)frame->cb % wbytes) == 0 &&
+    const bool aligned = ((uintptr_t)frame->y % wbytes) == 0 && ((uintptr_t)frame->cb % wbytes) == 0 &&
         ((uintptr_t)frame->cr % wbytes) == 0 && frame->stride_y % 4 == 0 && frame->stride_c % 4 == 0;
     for (int vert = 1; vert >= 0 && n_planes; vert--) {
         if (aligned) {

@@ -8,7 +8,7 @@
 //     keyed by (host object, picture number): a picture is uploaded once and then serves as reference for the pictures
 //     that follow it (EbPaReferenceObject lifetime, EbPictureBufferDesc.c:65-78 layout);
 //   * per-call slots (stream + device scratch/outputs + pinned staging) so N threads run N pictures at once;
-//   * the deblock -> CDEF search -> (host strength decision) -> CDEF apply chain of one picture with the
+//   * the deblock -> CDEF search -> strength decision -> CDEF apply chain of one picture with the
 //     reconstruction resident on the device across the stages.
 // What costs in this setting is not the GPU work of a picture but CUDA calls that take process-wide locks while ~20
 // pipeline threads are inside the library — cudaHostRegister of the caller's buffers (4 ms each and it stalls every other thread), cudaMalloc (device
@@ -22,7 +22,6 @@
 #include <condition_variable>
 #include <mutex>
 #include <thread>
-#include <sys/resource.h>
 #include <vector>
 
 #include "common.cuh"
@@ -101,8 +100,7 @@ struct SvtB200Engine {
     uint8_t *me_dev = nullptr, *me_pin = nullptr, *filt_dev = nullptr, *filt_pin = nullptr;
     struct {
         std::atomic<uint64_t> me_pictures{0}, dlf_frames{0}, cdef_frames{0}, lr_frames{0}, me_plane_uploads{0}, me_plane_hits{0}, h2d_bytes{0},
-            d2h_bytes{0}, pinned_bytes{0}, ns_slot_wait{0}, ns_pin{0}, ns_plane_wait{0}, ns_issue{0}, ns_sync{0}, ns_host_copy{0},
-            pin_calls{0};
+            d2h_bytes{0}, pinned_bytes{0}, ns_slot_wait{0}, ns_plane_wait{0}, ns_issue{0}, ns_sync{0}, ns_host_copy{0};
     } stats;
 };
 
@@ -268,21 +266,19 @@ int ensure_filt(SvtB200Engine *e, int w, int h, int bd, int mi_rows, int mi_cols
     return SVT_B200_OK;
 }
 
-// memcpy split over four threads above 4 MB (see run_copies below)
-// copies at or below this size stay on the calling thread (SVT_B200_COPY_MIN_KB; thread creation costs ~50 us)
-size_t copy_split_bytes() {
-    static const size_t v = getenv("SVT_B200_COPY_MIN_KB") ? (size_t)atol(getenv("SVT_B200_COPY_MIN_KB")) << 10 : (size_t)4 << 20;
-    return v;
-}
+// memcpy split over kCopyThreads threads above kCopySplitBytes (see run_copies below); smaller copies stay on the
+// calling thread (thread creation costs ~50 us)
+constexpr size_t kCopySplitBytes = (size_t)4 << 20;
+constexpr int kCopyThreads = 4;
 
 void par_memcpy(void *dst, const void *src, size_t n) {
-    if (n <= copy_split_bytes()) {
+    if (n <= kCopySplitBytes) {
         memcpy(dst, src, n);
         return;
     }
-    const size_t q = ((n / 4) + 4095) & ~(size_t)4095;
-    std::thread th[3];
-    for (int t = 1; t < 4; t++) {
+    const size_t q = ((n / kCopyThreads) + 4095) & ~(size_t)4095;
+    std::thread th[kCopyThreads - 1];
+    for (int t = 1; t < kCopyThreads; t++) {
         const size_t o = q * t, len = o >= n ? 0 : std::min(q, n - o);
         th[t - 1] = std::thread([=] {
             if (len) memcpy((uint8_t *)dst + o, (const uint8_t *)src + o, len);
@@ -409,30 +405,7 @@ void run_copies(SvtB200Engine *e, const RowCopy (&c)[3]) {
     Lap lap(e->stats.ns_host_copy);
     size_t total = 0;
     for (const RowCopy &k : c) total += k.bytes * k.rows;
-    static const int trace = getenv("SVT_B200_ENGINE_TRACE") ? atoi(getenv("SVT_B200_ENGINE_TRACE")) : 0;
-    static const int max_threads = getenv("SVT_B200_COPY_THREADS") ? atoi(getenv("SVT_B200_COPY_THREADS")) : 4;
-    const uint64_t t0 = trace ? now_ns() : 0;
-    struct Tr {
-        uint64_t t0;
-        size_t n;
-        int to_host;
-        rusage r0;
-        ~Tr() {
-            if (!t0) return;
-            rusage r1;
-            getrusage(RUSAGE_THREAD, &r1);
-            fprintf(stderr, "engine trace: picture copy %s %.1f MB in %.3f ms (minflt %ld majflt %ld nvcsw %ld nivcsw %ld cpu %.3f ms)\n",
-                    to_host ? "pinned->host" : "host->pinned", n / 1e6, (now_ns() - t0) / 1e6, r1.ru_minflt - r0.ru_minflt,
-                    r1.ru_majflt - r0.ru_majflt, r1.ru_nvcsw - r0.ru_nvcsw, r1.ru_nivcsw - r0.ru_nivcsw,
-                    ((r1.ru_utime.tv_sec - r0.ru_utime.tv_sec) + (r1.ru_stime.tv_sec - r0.ru_stime.tv_sec)) * 1e3 +
-                        ((r1.ru_utime.tv_usec - r0.ru_utime.tv_usec) + (r1.ru_stime.tv_usec - r0.ru_stime.tv_usec)) / 1e3);
-        }
-    } tr{t0, total, 0, {}};
-    if (trace) {
-        getrusage(RUSAGE_THREAD, &tr.r0);
-        tr.to_host = c[0].dst_pitch != c[0].bytes; // unpack writes strided host rows
-    }
-    const int nt = total > copy_split_bytes() ? std::max(1, std::min(8, max_threads)) : 1;
+    const int nt = total > kCopySplitBytes ? kCopyThreads : 1;
     auto part = [&c, nt](int t) {
         for (const RowCopy &k : c) copy_rows(k, (int)((int64_t)k.rows * t / nt), (int)((int64_t)k.rows * (t + 1) / nt));
     };
@@ -440,7 +413,7 @@ void run_copies(SvtB200Engine *e, const RowCopy (&c)[3]) {
         part(0);
         return;
     }
-    std::thread th[7];
+    std::thread th[kCopyThreads - 1];
     for (int t = 1; t < nt; t++) th[t - 1] = std::thread(part, t);
     part(0);
     for (int t = 1; t < nt; t++) th[t - 1].join();
@@ -550,12 +523,10 @@ int svt_b200_engine_get_stats(SvtB200Engine *e, SvtB200EngineStats *out) {
     out->d2h_bytes = e->stats.d2h_bytes;
     out->pinned_bytes = e->stats.pinned_bytes;
     out->ns_slot_wait = e->stats.ns_slot_wait;
-    out->ns_pin = e->stats.ns_pin;
     out->ns_plane_wait = e->stats.ns_plane_wait;
     out->ns_issue = e->stats.ns_issue;
     out->ns_sync = e->stats.ns_sync;
     out->ns_host_copy = e->stats.ns_host_copy;
-    out->pin_calls = e->stats.pin_calls;
     return SVT_B200_OK;
 }
 
@@ -875,127 +846,9 @@ int svt_b200_engine_lr_frame(SvtB200Engine *e, const SvtB200LrFrameParams *p, co
     return rc;
 }
 
-int svt_b200_engine_cdef_frame(SvtB200Engine *e, const SvtB200CdefSearchParams *sp, const SvtB200Frame *recon,
-                               const SvtB200Frame *source, const uint8_t *skip8, int32_t skip_stride, uint64_t *mse,
-                               SvtB200CdefDecideFn decide, void *user) {
-    return svt_b200_engine_dlf_cdef_frame(e, nullptr, nullptr, sp, recon, source, skip8, skip_stride, mse, decide, user);
-}
-
-int svt_b200_engine_dlf_cdef_frame(SvtB200Engine *e, const SvtB200DlfParams *dlf, const SvtB200DlfMi *mi,
-                                   const SvtB200CdefSearchParams *sp, const SvtB200Frame *recon, const SvtB200Frame *source,
-                                   const uint8_t *skip8, int32_t skip_stride, uint64_t *mse, SvtB200CdefDecideFn decide, void *user) {
-    if (!e || !sp || !recon || !source || !skip8 || !mse || !decide || recon->width != source->width ||
-        recon->height != source->height || recon->bit_depth != source->bit_depth || (dlf && (!mi || dlf->mi_stride != dlf->mi_cols))) {
-        set_error("svt_b200_engine_dlf_cdef_frame: bad argument");
-        return SVT_B200_ERR_ARG;
-    }
-    DeviceGuard dg(e->device);
-    int rc = ensure_filt(e, recon->width, recon->height, recon->bit_depth, sp->mi_rows, sp->mi_cols);
-    if (rc != SVT_B200_OK) return rc;
-    const FiltGeom &g = e->fg;
-    const int nvfb = (sp->mi_rows + 15) / 16, nhfb = (sp->mi_cols + 15) / 16, nfb = nvfb * nhfb;
-    const size_t b_skip = (size_t)((sp->mi_rows + 1) / 2) * skip_stride, b_mse = (size_t)2 * nfb * 64 * 8;
-    if (al256(b_skip) > g.skip || (size_t)nfb > g.nfb) {
-        set_error("svt_b200_engine_cdef_frame: skip map / filter-block count larger than the sequence geometry");
-        return SVT_B200_ERR_ARG;
-    }
-    const size_t b_mi = dlf ? (size_t)dlf->mi_rows * dlf->mi_cols * sizeof(SvtB200DlfMi) : 0;
-    if (b_mi > g.mi) {
-        set_error("svt_b200_engine_dlf_cdef_frame: mode-info array larger than the sequence geometry");
-        return SVT_B200_ERR_ARG;
-    }
-    FiltSlot *s = acquire(e, e->filt);
-    do {
-        uint8_t *d_small = s->misc + g.mi + 4096; // the mode-info summary (deblocking) occupies the head of misc
-        uint8_t *d_skip = d_small, *d_mse = d_small + g.skip, *d_idx = d_mse + g.mse;
-        uint8_t *h_skip = s->pin_small, *h_mse = h_skip + g.skip, *h_idx = h_mse + g.mse;
-        pack_frame(e, s->pin_a, recon);
-        if (dlf) { // the deblocking the DLF stage deferred: same upload of the reconstruction serves both filters
-            {
-                Lap lap(e->stats.ns_host_copy);
-                par_memcpy(s->pin_b, mi, b_mi);
-            }
-            Lap lap(e->stats.ns_issue);
-            if (cudaMemcpyAsync(s->misc, s->pin_b, b_mi, cudaMemcpyHostToDevice, s->st) != cudaSuccess) {
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            if ((rc = copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st)) != SVT_B200_OK) break;
-            if ((rc = svt_b200_dlf_frame(dlf, &s->recon, (const SvtB200DlfMi *)s->misc, s->st)) != SVT_B200_OK) break;
-            if (timed_sync(e, s->st) != cudaSuccess) { // pin_b is reused for the source picture below
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            e->stats.dlf_frames++;
-            e->stats.h2d_bytes += b_mi;
-        }
-        pack_frame(e, s->pin_b, source);
-        memcpy(h_skip, skip8, b_skip);
-        {
-            Lap lap(e->stats.ns_issue);
-            if (cudaMemcpyAsync(d_skip, h_skip, b_skip, cudaMemcpyHostToDevice, s->st) != cudaSuccess) {
-                set_error("engine: skip-map upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            if (!dlf && (rc = copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st)) != SVT_B200_OK) break;
-            if ((rc = copy_packed(e, &s->source, s->pin_b, cudaMemcpyHostToDevice, s->st)) != SVT_B200_OK) break;
-            if ((rc = svt_b200_cdef_search(sp, &s->recon, &s->source, d_skip, skip_stride, (uint64_t *)d_mse, s->st)) != SVT_B200_OK)
-                break;
-            if (cudaMemcpyAsync(h_mse, d_mse, b_mse, cudaMemcpyDeviceToHost, s->st) != cudaSuccess) {
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-        }
-        if (timed_sync(e, s->st) != cudaSuccess) {
-            set_error("engine: CDEF search failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = SVT_B200_ERR_CUDA;
-            break;
-        }
-        memcpy(mse, h_mse, b_mse);
-        // the strength decision (finish_cdef_search, EbEncCdef.c:1167) is the host's: it reads mse and fills the apply set
-        SvtB200CdefApplyParams ap;
-        memset(&ap, 0, sizeof(ap));
-        ap.mi_rows = sp->mi_rows;
-        ap.mi_cols = sp->mi_cols;
-        int8_t *idx = (int8_t *)h_idx;
-        memset(idx, -1, (size_t)nfb);
-        const int apply = decide(user, mse, &ap, idx);
-        e->stats.cdef_frames++;
-        e->stats.h2d_bytes += b_skip;
-        e->stats.d2h_bytes += b_mse;
-        if (apply <= 0) {
-            if (apply < 0) {
-                set_error("svt_b200_engine_cdef_frame: the strength-decision callback failed");
-                rc = SVT_B200_ERR_ARG;
-            }
-            break;
-        }
-        {
-            Lap lap(e->stats.ns_issue);
-            if (cudaMemcpyAsync(d_idx, idx, (size_t)nfb, cudaMemcpyHostToDevice, s->st) != cudaSuccess) {
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            if ((rc = svt_b200_cdef_apply(&ap, &s->recon, &s->out, d_skip, skip_stride, (const int8_t *)d_idx, s->st)) != SVT_B200_OK)
-                break;
-            if ((rc = copy_packed(e, &s->out, s->pin_a, cudaMemcpyDeviceToHost, s->st)) != SVT_B200_OK) break;
-        }
-        if (timed_sync(e, s->st) != cudaSuccess) {
-            set_error("engine: CDEF apply failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = SVT_B200_ERR_CUDA;
-            break;
-        }
-        unpack_frame(e, recon, s->pin_a);
-    } while (0);
-    if (rc != SVT_B200_OK) cudaStreamSynchronize(s->st);
-    release(e, s);
-    return rc;
-}
-
-// The same picture pass with the strength decision on the DEVICE (svt_b200_cdef_decide replaces the host callback): one
-// upload, deblocking, CDEF search, decision, CDEF apply, one download, ONE synchronisation - the reconstruction and the
-// decision arrive together.  apply: 0 = search + decision only (EbCdefProcess.c:527-529: nobody reads the filtered picture).
+// The CDEF stage of one picture, with the deblocking the DLF stage deferred (dlf != NULL) and the strength decision on
+// the device (svt_b200_cdef_decide): one upload, deblocking, CDEF search, decision, CDEF apply, one download, ONE
+// synchronisation - the reconstruction and the decision arrive together.  apply: 0 = search + decision only (EbCdefProcess.c:527-529: nobody reads the filtered picture).
 int svt_b200_engine_dlf_cdef_frame_dev(SvtB200Engine *e, const SvtB200DlfParams *dlf, const SvtB200DlfMi *mi,
                                        const SvtB200CdefSearchParams *sp, const SvtB200CdefDecideParams *dp, int32_t damping,
                                        int32_t apply, const SvtB200Frame *recon, const SvtB200Frame *source, const uint8_t *skip8,

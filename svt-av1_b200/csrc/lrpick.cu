@@ -7,13 +7,9 @@
 // compute_stats builds the Wiener normal equations of one restoration unit: with y = the win x win window of the
 // degraded picture around a sample (minus the unit average, column-major: idx = (dx+hw)*win + (dy+hw)) and x = the
 // source sample (minus the average), M[k] = sum y[k] x and H[k][l] = sum y[k] y[l] over the unit (int64, exact).
-// That is 49*50/2 + 49 multiply-accumulates per luma sample — integer work with exact 64-bit sums, so it runs on the
-// integer pipes, not on tensor cores.  Decomposition: a CTA owns a 32x16 sample tile of one unit (staged once with
-// its halo as int16 differences); H is cut into win x win blocks "window column kc x window column lc" (28 block pairs
-// for win 7) and a thread owns one block pair for a 1/8 subset of the tile's samples: 2*win LDS feed win*win IMAD into
-// register accumulators (int32 is safe for the <= 64 samples a thread sees, also at 12 bit).  Threads of a CTA merge
-// through shared-memory int32 atomics, CTAs through one 64-bit global atomic per entry.  The linear solves of the
-// search stay on the host (double precision, tiny), as in SURVEY.md §8(a).
+// Three kernels: stats_sum_kernel (the unit averages), stats_mma_kernel (M and H on the INT8 tensor cores, exact: see
+// its comment) and stats_finish_kernel (high-bit-depth divider, mirror of H).  The linear solves of the search stay on
+// the host (double precision, tiny), as in SURVEY.md §8(a).
 #include <algorithm>
 
 #include "common.cuh"
@@ -21,8 +17,6 @@
 using namespace svtb200;
 
 namespace {
-
-constexpr int ST_TW = 32, ST_TH = 16, ST_NT = 256;
 
 struct StatsUnit { // one restoration unit of a plane
     int h_start, h_end, v_start, v_end;
@@ -52,93 +46,7 @@ __global__ void __launch_bounds__(256) stats_sum_kernel(const StatsDev d) {
     if ((threadIdx.x & 31) == 0 && acc) atomicAdd(&d.sum[blockIdx.y], acc);
 }
 
-template <typename T, int WIN>
-__global__ void __launch_bounds__(ST_NT) stats_kernel(const StatsDev d, int tiles_x_max) {
-    constexpr int HW = WIN / 2, WIN2 = WIN * WIN, TW = ST_TW + 2 * HW, TH = ST_TH + 2 * HW;
-    constexpr int NPAIR = WIN * (WIN + 1) / 2, NSUB = (ST_NT - 32) / NPAIR; // 28 pairs x 8 sample subsets (win 7)
-    __shared__ int16_t s_y[TH * TW];
-    __shared__ int16_t s_x[ST_TH * ST_TW];
-    __shared__ unsigned long long s_acc[WIN2 + WIN2 * WIN2]; // 64-bit: a 512-sample tile overflows int32 at 12 bit
-    const StatsUnit u = d.units[blockIdx.y];
-    const int uw = u.h_end - u.h_start, uh = u.v_end - u.v_start;
-    const int tx = blockIdx.x % tiles_x_max, ty = blockIdx.x / tiles_x_max;
-    const int x0 = u.h_start + tx * ST_TW, y0 = u.v_start + ty * ST_TH;
-    if (x0 >= u.h_end || y0 >= u.v_end) return;
-    const int tw = min(ST_TW, u.h_end - x0), th = min(ST_TH, u.v_end - y0);
-    const int avg = (int)(d.sum[blockIdx.y] / (unsigned long long)(uw * uh)); // find_average: truncating division
-    const T *dg = reinterpret_cast<const T *>(d.dgd);
-    const T *sr = reinterpret_cast<const T *>(d.src);
-    const int tid = threadIdx.x;
-    for (int i = tid; i < TH * TW; i += ST_NT) {
-        const int r = i / TW, c = i - r * TW;
-        int yy = y0 + r - HW, xx = x0 + c - HW;
-        if (d.clamp) {
-            yy = min(max(yy, 0), d.ph - 1);
-            xx = min(max(xx, 0), d.pw - 1);
-        }
-        const bool need = r < th + 2 * HW && c < tw + 2 * HW;
-        s_y[i] = need ? (int16_t)((int)dg[(size_t)yy * d.dgd_stride + xx] - avg) : (int16_t)0;
-    }
-    for (int i = tid; i < ST_TH * ST_TW; i += ST_NT) {
-        const int r = i / ST_TW, c = i - r * ST_TW;
-        s_x[i] = (r < th && c < tw) ? (int16_t)((int)sr[(size_t)(y0 + r) * d.src_stride + x0 + c] - avg) : (int16_t)0;
-    }
-    for (int i = tid; i < WIN2 + WIN2 * WIN2; i += ST_NT) s_acc[i] = 0;
-    __syncthreads();
-    if (tid < NPAIR * NSUB) { // H: block pair (kc <= lc), sample subset `sub`
-        const int pair = tid % NPAIR, sub = tid / NPAIR;
-        int kc = 0, rem = pair; // pair -> (kc, lc), kc <= lc
-        while (rem >= WIN - kc) {
-            rem -= WIN - kc;
-            kc++;
-        }
-        const int lc = kc + rem;
-        int acc[WIN][WIN];
-#pragma unroll
-        for (int a = 0; a < WIN; a++)
-#pragma unroll
-            for (int b = 0; b < WIN; b++) acc[a][b] = 0;
-        for (int px = sub; px < th * tw; px += NSUB) {
-            const int pi = px / tw, pj = px - pi * tw;
-            int yk[WIN], yl[WIN];
-#pragma unroll
-            for (int a = 0; a < WIN; a++) {
-                yk[a] = s_y[(pi + a) * TW + pj + kc];
-                yl[a] = s_y[(pi + a) * TW + pj + lc];
-            }
-#pragma unroll
-            for (int a = 0; a < WIN; a++)
-#pragma unroll
-                for (int b = 0; b < WIN; b++) acc[a][b] += yk[a] * yl[b];
-        }
-#pragma unroll
-        for (int a = 0; a < WIN; a++)
-#pragma unroll
-            for (int b = 0; b < WIN; b++) {
-                const int k = kc * WIN + a, l = lc * WIN + b;
-                if (l >= k && acc[a][b]) atomicAdd(&s_acc[WIN2 + k * WIN2 + l], (unsigned long long)(long long)acc[a][b]);
-            }
-    } else if (tid >= ST_NT - 32) { // M: the last warp
-        const int lane = tid & 31;
-        for (int k = lane; k < WIN2; k += 32) {
-            const int kcol = k / WIN, krow = k - kcol * WIN;
-            long long acc = 0;
-            for (int px = 0; px < th * tw; px++) {
-                const int pi = px / tw, pj = px - pi * tw;
-                acc += (int)s_y[(pi + krow) * TW + pj + kcol] * (int)s_x[pi * ST_TW + pj];
-            }
-            s_acc[k] = (unsigned long long)acc;
-        }
-    }
-    __syncthreads();
-    long long *out = d.out + (size_t)blockIdx.y * (WIN2 + WIN2 * WIN2);
-    for (int i = tid; i < WIN2 + WIN2 * WIN2; i += ST_NT) {
-        const unsigned long long v = s_acc[i];
-        if (v) atomicAdd(reinterpret_cast<unsigned long long *>(out + i), v);
-    }
-}
-
-// ---- the same normal equations on the INT8 tensor cores ---------------------------------------------------------
+// ---- the normal equations on the INT8 tensor cores ------------------------------------------------------------
 // H and M together are the Gram matrix of z = [the win2 window differences, the source difference] over the samples of
 // a unit: G = Z^T Z (upper triangle; column win2 is M).  The differences need 9 (8-bit) to 13 (12-bit) bits, the tensor
 // cores multiply int8, so every difference is split once, at staging, into balanced limbs  v = 128 * hi + lo,
@@ -168,8 +76,9 @@ __device__ __forceinline__ void mma_s8(int (&c)[4], uint32_t a0, uint32_t a1, ui
                  : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
-template <typename T, int WIN, int MINB>
-__global__ void __launch_bounds__(TC_NT, MINB) stats_mma_kernel(const StatsDev d, int tiles_x_max) {
+// One resident CTA per SM: a register cap for two (80 registers) spills the accumulators and runs slower.
+template <typename T, int WIN>
+__global__ void __launch_bounds__(TC_NT, 1) stats_mma_kernel(const StatsDev d, int tiles_x_max) {
     constexpr int HW = WIN / 2, WIN2 = WIN * WIN, NROW = WIN2 + 1, NJ = (NROW + 7) / 8, MT = (NJ + 1) / 2;
     constexpr int RH = TC_TH + 2 * HW, YB = RH * TC_PITCH, XB = TC_TH * TC_XPITCH, SW = TC_XPITCH / 4; // SW: staged words per row
     constexpr int NTILE = MT * NJ - MT * (MT - 1); // sum over mt of (NJ - 2 mt): column tiles nt >= 2 mt
@@ -320,54 +229,21 @@ int stats_launch(StatsDev &d, int win, int hbd, int max_uw, int max_uh, cudaStre
     const int win2 = win * win;
     if (cudaMemsetAsync(d.sum, 0, (size_t)d.n_units * 8, st) != cudaSuccess) return -1;
     if (cudaMemsetAsync(d.out, 0, (size_t)d.n_units * (win2 + win2 * win2) * 8, st) != cudaSuccess) return -1;
-    // SVT_B200_STATS_IMAD=1: the round-1 integer-pipe kernel (kept for the comparison with the tensor-core kernel)
-    static const bool imad = getenv("SVT_B200_STATS_IMAD") != nullptr;
     const dim3 gs(std::min(64, (max_uw * max_uh + 255) / 256), d.n_units);
-    if (!imad) {
-        // SVT_B200_STATS_MINB=2: the register-capped build of the same kernel (80 registers, 2 CTAs / SM, some spills).
-        // Measured slower (1080p 0.134 vs 0.105 ms, 2160p 10-bit 0.423 vs 0.344 ms): the spilled accumulators cost more than
-        // the second resident CTA hides - kept selectable for that comparison only.
-        static const bool two = getenv("SVT_B200_STATS_MINB") && atoi(getenv("SVT_B200_STATS_MINB")) == 2;
-        const int tiles_x = (max_uw + TC_TW - 1) / TC_TW, tiles_y = (max_uh + TC_TH - 1) / TC_TH;
-        const dim3 gt(tiles_x * tiles_y, d.n_units);
-#define SVTB_STATS_MMA(T, W)                                                                  \
-    do {                                                                                      \
-        if (two)                                                                              \
-            SVTB_LAUNCH((stats_mma_kernel<T, W, 2>), gt, TC_NT, 0, st, d, tiles_x);           \
-        else                                                                                  \
-            SVTB_LAUNCH((stats_mma_kernel<T, W, 1>), gt, TC_NT, 0, st, d, tiles_x);           \
-    } while (0)
-        if (hbd) {
-            SVTB_LAUNCH(stats_sum_kernel<uint16_t>, gs, 256, 0, st, d);
-            if (win == 7)
-                SVTB_STATS_MMA(uint16_t, 7);
-            else
-                SVTB_STATS_MMA(uint16_t, 5);
-        } else {
-            SVTB_LAUNCH(stats_sum_kernel<uint8_t>, gs, 256, 0, st, d);
-            if (win == 7)
-                SVTB_STATS_MMA(uint8_t, 7);
-            else
-                SVTB_STATS_MMA(uint8_t, 5);
-        }
-#undef SVTB_STATS_MMA
-        SVTB_LAUNCH(stats_finish_kernel, d.n_units, 256, 0, st, d.out, d.n_units, win2, d.divider);
-        return cudaGetLastError() == cudaSuccess ? 0 : -1;
-    }
-    const int tiles_x = (max_uw + ST_TW - 1) / ST_TW, tiles_y = (max_uh + ST_TH - 1) / ST_TH;
+    const int tiles_x = (max_uw + TC_TW - 1) / TC_TW, tiles_y = (max_uh + TC_TH - 1) / TC_TH;
     const dim3 gt(tiles_x * tiles_y, d.n_units);
     if (hbd) {
         SVTB_LAUNCH(stats_sum_kernel<uint16_t>, gs, 256, 0, st, d);
         if (win == 7)
-            SVTB_LAUNCH((stats_kernel<uint16_t, 7>), gt, ST_NT, 0, st, d, tiles_x);
+            SVTB_LAUNCH((stats_mma_kernel<uint16_t, 7>), gt, TC_NT, 0, st, d, tiles_x);
         else
-            SVTB_LAUNCH((stats_kernel<uint16_t, 5>), gt, ST_NT, 0, st, d, tiles_x);
+            SVTB_LAUNCH((stats_mma_kernel<uint16_t, 5>), gt, TC_NT, 0, st, d, tiles_x);
     } else {
         SVTB_LAUNCH(stats_sum_kernel<uint8_t>, gs, 256, 0, st, d);
         if (win == 7)
-            SVTB_LAUNCH((stats_kernel<uint8_t, 7>), gt, ST_NT, 0, st, d, tiles_x);
+            SVTB_LAUNCH((stats_mma_kernel<uint8_t, 7>), gt, TC_NT, 0, st, d, tiles_x);
         else
-            SVTB_LAUNCH((stats_kernel<uint8_t, 5>), gt, ST_NT, 0, st, d, tiles_x);
+            SVTB_LAUNCH((stats_mma_kernel<uint8_t, 5>), gt, TC_NT, 0, st, d, tiles_x);
     }
     SVTB_LAUNCH(stats_finish_kernel, d.n_units, 256, 0, st, d.out, d.n_units, win2, d.divider);
     return cudaGetLastError() == cudaSuccess ? 0 : -1;

@@ -214,11 +214,8 @@ class HostLrLines(C.Structure):  # SvtB200HostLrLines
 
 class EngineStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("me_pictures", "dlf_frames", "cdef_frames", "lr_frames", "me_plane_uploads", "me_plane_hits",
-                                          "h2d_bytes", "d2h_bytes", "pinned_bytes", "ns_slot_wait", "ns_pin", "ns_plane_wait", "ns_issue",
-                                          "ns_sync", "ns_host_copy", "pin_calls")]
-
-
-CDEF_DECIDE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(CdefApplyParams), C.POINTER(C.c_int8))
+                                          "h2d_bytes", "d2h_bytes", "pinned_bytes", "ns_slot_wait", "ns_plane_wait", "ns_issue",
+                                          "ns_sync", "ns_host_copy")]
 
 
 def preset8_me_params(width, height, n_l0=1, n_l1=1, dist=((1, 2, 3, 4), (1, 2, 3, 4)), temporal_layer=1,

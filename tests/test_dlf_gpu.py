@@ -89,6 +89,27 @@ def test_dlf_frame_vs_oracle(case):
         np.testing.assert_array_equal(same.plane(i), frame.plane(i))
 
 
+@pytest.mark.parametrize("case", DLF_CASES[:2])
+def test_dlf_frame_misaligned_planes_vs_oracle(case):
+    """Planes whose base and stride are not multiples of 4 samples (pad 17) take the line-per-thread kernel."""
+    import gpu_runner as gr
+    w, h, bd, seed, levels, sharp = case
+    mi_rows, mi_cols, part, aligned = dlf_case(w, h, bd, seed, levels, sharp)
+    frame = cm.Yuv(w, h, bd, pad=17)
+    for i in range(3):
+        frame.plane(i)[...] = aligned.plane(i)
+    st = frame.struct()
+    assert st.stride_y % 4 and st.stride_c % 4
+    flat = flat_mi(mi_rows, mi_cols, part, levels)
+    p = dlf_params(mi_rows, mi_cols, levels, sharp)
+    want = frame.copy()
+    ws = want.struct()
+    cm.oracle().orc_dlf_frame(C.byref(p), C.byref(ws), flat)
+    got = gr.run_gpu_dlf(p, frame, flat)
+    for i in range(3):
+        np.testing.assert_array_equal(got.plane(i), want.plane(i), err_msg=f"plane {i}")
+
+
 def test_frame_sse():
     import gpu_runner as gr
     for (w, h, bd) in ((192, 136, 8), (640, 360, 10), (1920, 1080, 8)):

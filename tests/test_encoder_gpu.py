@@ -60,16 +60,6 @@ def test_360p_preset8_device_side_me_downsample(tmp_path):
 
 
 @skip_if_unbuilt
-def test_360p_cdef_strength_decision_on_the_host(tmp_path):
-    """SVT_CUDA_CDEF_DECIDE=0: the CDEF call keeps the reference's finish_cdef_search on the host (the engine's callback form);
-    the default runs the decision on the device (svt_b200_cdef_decide).  Both must give the C encoder's stream."""
-    clip = _clip(tmp_path, 640, 360, 20, 8)
-    ref = ec.run_variant("ref_c", clip, 640, 360, 20, 8, 50, 8, str(tmp_path))
-    gpu = ec.run_variant("cuda_c", clip, 640, 360, 20, 8, 50, 8, str(tmp_path), extra_env={"SVT_CUDA_CDEF_DECIDE": "0"})
-    _same(ref, gpu)
-
-
-@skip_if_unbuilt
 def test_10bit_preset6_bitstream_and_recon_md5(tmp_path):
     """A 10-bit preset-6 clip (the configs[2] stage set at a small size): 16-bit pipeline, loop_filter_mode 3 (level search +
     deblocking in dlf_kernel as one GPU call), CDEF on 16-bit planes, restoration search on the CPU and apply on the GPU."""

@@ -85,7 +85,7 @@ def main():
     ap.add_argument("--no-recon", action="store_true")
     ap.add_argument("--profile", action="store_true")
     ap.add_argument("--workdir", default=None)
-    ap.add_argument("--env", action="append", default=[], help="KEY=VALUE passed to the encoders (e.g. SVT_CUDA_CDEF_DECIDE=0)")
+    ap.add_argument("--env", action="append", default=[], help="KEY=VALUE passed to the encoders (e.g. SVT_CUDA_ME_DS=1)")
     a = ap.parse_args()
     wd = a.workdir or tempfile.mkdtemp(prefix="svtenc_", dir="/dev/shm" if os.path.isdir("/dev/shm") else None)
     os.makedirs(wd, exist_ok=True)

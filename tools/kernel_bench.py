@@ -105,10 +105,6 @@ def geometry(w, h, bd):
     alg = 2 * (2 * pic_bytes) + 2 * mi_rows * mi_cols * 16
     out["rows"].append(row("svt_b200_dlf_frame (2 launches: all vertical edges, all horizontal edges)", ms, alg, copy_ms,
                            "2 passes x (read + write) + the 16 B / 4x4 mode-info summary per pass"))
-    os.environ["SVT_B200_DLF_LINE_KERNEL"] = "1"
-    ms_old = ring_ms(call, ring, restore)
-    del os.environ["SVT_B200_DLF_LINE_KERNEL"]
-    out["rows"].append(row("  (round-1 kernel: one thread per sample line, scalar accesses)", ms_old, alg, copy_ms))
     del dfs, dmis, pristine
 
     # ---- CDEF --------------------------------------------------------------------------------------------------

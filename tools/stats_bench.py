@@ -1,21 +1,20 @@
 #!/usr/bin/env python
-"""svt_b200_lr_wiener_stats (all compute_stats calls of search_wiener for a luma plane, win 7): the INT8 tensor-core
-kernel (default) against the round-1 integer-pipe kernel (SVT_B200_STATS_IMAD=1) at the two bench geometries.  The kernel
-choice is read once per process, so the script runs itself once per kernel.  Device time with CUDA events over 20 calls
-after 3 warm-up calls (the pictures, 3 MB / 25 MB, stay in L2: the kernels are arithmetic bound, see the MAC rates).
+"""svt_b200_lr_wiener_stats (all compute_stats calls of search_wiener for a luma plane, win 7; the INT8 tensor-core
+kernel) at the two bench geometries.  Device time with CUDA events over 20 calls after 3 warm-up calls (the pictures,
+3 MB / 25 MB, stay in L2: the kernel is arithmetic bound, see the MAC rates).  The checksum of each row is the XOR of
+the returned statistics.
 
     python tools/stats_bench.py > gpurun_out/stats_bench.json
 """
 import ctypes as C
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def child():
+def main():
     for p in (os.path.join(ROOT, "svt-av1_b200"), os.path.join(ROOT, "tests")):
         sys.path.insert(0, p)
     import numpy as np
@@ -51,20 +50,8 @@ def child():
         rows.append({"geometry": "%dx%d %d-bit luma, %d units of %d" % (W, H, bd, len(rects), unit), "ms": round(ms, 4),
                      "useful_int_macs": macs, "useful_tmacs": round(macs / ms / 1e9, 2),
                      "checksum": int(np.bitwise_xor.reduce(h))})
-    print(json.dumps(rows))
+    print(json.dumps({"device": torch.cuda.get_device_name(), "rows": rows}, indent=1))
 
 
 if __name__ == "__main__":
-    if len(sys.argv) > 1 and sys.argv[1] == "--child":
-        child()
-        sys.exit(0)
-    out = {}
-    for name, env in (("int8_tensor_core (IMMA.16832.S8, default)", {}), ("integer_pipe (round 1, SVT_B200_STATS_IMAD=1)", {"SVT_B200_STATS_IMAD": "1"})):
-        e = dict(os.environ)
-        e.update(env)
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child"], env=e, stdout=subprocess.PIPE, timeout=900)
-        out[name] = json.loads(r.stdout.decode().strip().splitlines()[-1])
-    a, b = list(out.values())
-    out["speedup"] = [round(y["ms"] / x["ms"], 2) for x, y in zip(a, b)]
-    out["same_results"] = all(x["checksum"] == y["checksum"] for x, y in zip(a, b))
-    print(json.dumps(out, indent=1))
+    main()
