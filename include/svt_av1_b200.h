@@ -994,7 +994,8 @@ SVT_B200_API int svt_b200_engine_lr_frame(SvtB200Engine *e, const SvtB200LrFrame
  * block, the strength decision (svt_b200_cdef_decide: finish_cdef_search, EbEncCdef.c:1167), frame apply written back
  * into `recon` (host) in place when apply != 0, one download, ONE synchronisation.  With apply = 0 the host
  * reconstruction is left as it was: the reference does not filter a picture nobody reads.  decision / fb_strength_idx:
- * HOST outputs (frame header fields and mbmi.cdef_strength per filter block, -1 = all-skip block). */
+ * HOST outputs (frame header fields and mbmi.cdef_strength per filter block, -1 = all-skip block).  skip_stride up to
+ * ((mi_cols + 1) / 2 + 15) & ~15 fits the engine's staging of the skip map; a larger stride may return SVT_B200_ERR_ARG. */
 SVT_B200_API int svt_b200_engine_dlf_cdef_frame_dev(SvtB200Engine *e, const SvtB200DlfParams *dlf, const SvtB200DlfMi *mi,
                                                     const SvtB200CdefSearchParams *sp, const SvtB200CdefDecideParams *dp,
                                                     int32_t damping, int32_t apply, const SvtB200Frame *recon,

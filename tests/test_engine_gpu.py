@@ -29,19 +29,28 @@ def _host_pic(key, tag, planes, with_decimations=True):
     return h
 
 
-def test_engine_me_picture_residency_and_results():
-    """Three 'pictures' in coding order, each searched against the earlier ones: every call equals the oracle, and a picture
-    uploaded once (as source) is found resident when it is a reference later (the engine's counters)."""
+def assert_me_result(got, want, n_sb, what=""):
+    """The engine's four ME outputs against the oracle's; candidates beyond total_cand are unspecified."""
+    np.testing.assert_array_equal(got.me_mv, want.me_mv, err_msg=f"me_mv {what}")
+    np.testing.assert_array_equal(got.total_cand, want.total_cand, err_msg=f"total_cand {what}")
+    np.testing.assert_array_equal(got.rc, want.rc, err_msg=f"rc {what}")
+    used = np.arange(23) < want.total_cand[:, :, None].astype(np.int64)
+    np.testing.assert_array_equal(got.me_cand.reshape(n_sb, 85, 23)[used], want.me_cand.reshape(n_sb, 85, 23)[used],
+                                  err_msg=f"me_cand {what}")
+
+
+def run_me_steps(w, h, steps, uploads, hits):
+    """'Pictures' in coding order, each searched against the earlier ones on one engine: every call equals the oracle, and
+    the residency counters equal `uploads` / `hits`."""
     lib = sb.load()
     e = C.c_void_p()
     sb.check(lib.svt_b200_engine_create(0, C.byref(e)), lib)
     try:
-        w, h = 256, 192
         dist = ((1, 2, 3, 4), (1, 2, 3, 4))
         geos, src, refs = cm.make_me_case(w, h, 2, 2, seed=21)
         pics = [refs[1], refs[0], src, refs[4]]  # distinct contents; keys = their index
         n_sb = ((w + 63) // 64) * ((h + 63) // 64)
-        for step, (cur, l0, l1) in enumerate([(1, [0], []), (2, [1, 0], []), (3, [2, 1], [0])]):
+        for step, (cur, l0, l1) in enumerate(steps):
             params = sb.preset8_me_params(w, h, len(l0), len(l1), dist, 1, 1)
             want = cm.run_oracle_me(params, pics[cur], [pics[i] for i in l0] + [pics[0]] * (4 - len(l0)) + [pics[i] for i in l1] + [pics[0]] * (4 - len(l1)))
             hs = _host_pic(1000 + cur, cur, pics[cur])
@@ -53,19 +62,23 @@ def test_engine_me_picture_residency_and_results():
             got = cm.MeBuffers(n_sb)
             sb.check(lib.svt_b200_engine_me_picture(e, C.byref(params), C.byref(hs), hr, 1, cm.ptr(got.me_mv), cm.ptr(got.me_cand),
                                                     cm.ptr(got.total_cand), cm.ptr(got.rc)), lib)
-            np.testing.assert_array_equal(got.me_mv, want.me_mv, err_msg=f"me_mv step {step}")
-            np.testing.assert_array_equal(got.total_cand, want.total_cand)
-            np.testing.assert_array_equal(got.rc, want.rc)
-            for sbi in range(n_sb):  # candidates beyond total_cand are unspecified
-                for pu in range(85):
-                    n = int(want.total_cand[sbi, pu])
-                    np.testing.assert_array_equal(got.me_cand[sbi, pu * 23:pu * 23 + n], want.me_cand[sbi, pu * 23:pu * 23 + n])
+            assert_me_result(got, want, n_sb, f"step {step}")
         st = sb.EngineStats()
         sb.check(lib.svt_b200_engine_get_stats(e, C.byref(st)), lib)
-        assert st.me_pictures == 3
-        assert st.me_plane_uploads == 4 and st.me_plane_hits == 5  # 4 distinct pictures; 1+2+... reference re-uses found resident
+        assert st.me_pictures == len(steps)
+        assert st.me_plane_uploads == uploads and st.me_plane_hits == hits
     finally:
         lib.svt_b200_engine_destroy(e)
+
+
+def test_engine_me_picture_residency_and_results():
+    """A picture uploaded once (as source) is found resident when it is a reference later: 4 distinct pictures, 5 reuses."""
+    run_me_steps(256, 192, [(1, [0], []), (2, [1, 0], []), (3, [2, 1], [0])], 4, 5)
+
+
+def test_engine_me_picture_above_copy_split():
+    """3840x2160: the full plane (8.7 MB) is staged by the host copy split over threads; 2 list0 + 1 list1 references."""
+    run_me_steps(3840, 2160, [(3, [2, 1], [0])], 4, 0)
 
 
 def test_engine_me_device_side_downsample_matches_uploaded_planes():
@@ -98,7 +111,9 @@ def test_engine_me_device_side_downsample_matches_uploaded_planes():
         lib.svt_b200_engine_destroy(e)
 
 
-@pytest.mark.parametrize("case", [(320, 192, 8, 6, (12, 30, 0, 22), 2), (192, 136, 10, 2, (33, 17, 40, 25), 3)])
+# 1920x1080 10-bit: the packed picture (6.2 MB) is staged by the split host copy
+@pytest.mark.parametrize("case", [(320, 192, 8, 6, (12, 30, 0, 22), 2), (192, 136, 10, 2, (33, 17, 40, 25), 3),
+                                  (1920, 1080, 10, 7, (36, 28, 20, 14), 1)])
 def test_engine_dlf_frame(engine, case):
     from test_dlf_gpu import flat_mi
     from test_oracle_dlf import dlf_case, dlf_params
@@ -122,75 +137,100 @@ def test_engine_dlf_frame(engine, case):
         lib.svt_b200_engine_destroy(e)
 
 
-@pytest.mark.parametrize("bd,with_dlf,pick", [(8, False, 3), (10, False, 3), (10, True, 2), (8, True, 3)])
-def test_engine_cdef_frame_with_device_decision(bd, with_dlf, pick):
-    """deblocking -> search -> svt_b200_cdef_decide (finish_cdef_search on the device) -> apply in ONE engine call: the
-    decision, the per-filter-block choice and the filtered picture against the oracle chain."""
-    from test_dlf_gpu import flat_mi
-    from test_oracle_cdef import cdef_picture_case
-    from test_oracle_dlf import dlf_params
-    lib, orc = sb.load(), cm.oracle()
-    e = C.c_void_p()
-    sb.check(lib.svt_b200_engine_create(0, C.byref(e)), lib)
-    try:
-        w, h = 320, 200
-        src, rec, mi_rows, mi_cols, skip = cdef_picture_case(w, h, bd)
-        skip[0:8, 0:8] = 1  # one filter block entirely skipped
-        levels = (20, 24, 12, 9)
-        pre = rec.copy()
-        dp, flat = None, None
+class CdefChain:
+    """Inputs of one svt_b200_engine_dlf_cdef_frame_dev call and the oracle's chain on them: deblocking (with_dlf) ->
+    strength search -> finish_cdef_search -> apply (damping 5, lambda 3500)."""
+
+    def __init__(self, w, h, bd, with_dlf, pick, seed=9, part_seed=5, levels=(20, 24, 12, 9)):
+        from test_dlf_gpu import flat_mi
+        from test_oracle_cdef import cdef_picture_case
+        from test_oracle_dlf import dlf_params
+        lib, orc = sb.load(), cm.oracle()
+        self.src, self.rec, mi_rows, mi_cols, skip = cdef_picture_case(w, h, bd, seed)
+        # the engine stages skip maps up to the encoder's row stride: (mi_cols + 1) / 2 rounded up to 16
+        self.skip = np.ascontiguousarray(skip[:, :((mi_cols + 1) // 2 + 15) & ~15])
+        self.skip[0:8, 0:8] = 1  # one filter block entirely skipped
+        pre = self.rec.copy()
+        self.dp, self.flat = None, None
         if with_dlf:
-            part = cm.random_partition(mi_rows, mi_cols, 5)
-            flat = flat_mi(mi_rows, mi_cols, part, levels)
-            dp = dlf_params(mi_rows, mi_cols, levels, 1)
+            part = cm.random_partition(mi_rows, mi_cols, part_seed)
+            self.flat = flat_mi(mi_rows, mi_cols, part, levels)
+            self.dp = dlf_params(mi_rows, mi_cols, levels, 1)
             ps = pre.struct()
-            orc.orc_dlf_frame(C.byref(dp), C.byref(ps), flat)
-        sp = sb.CdefSearchParams()
+            orc.orc_dlf_frame(C.byref(self.dp), C.byref(ps), self.flat)
+        self.sp = sp = sb.CdefSearchParams()
         sp.mi_rows, sp.mi_cols, sp.pri_damping = mi_rows, mi_cols, 5
         orc.orc_cdef_strength_table(pick, C.byref(sp))
-        dcp = sb.CdefDecideParams()
+        self.dcp = dcp = sb.CdefDecideParams()
         assert lib.svt_b200_cdef_decide_table(pick, C.byref(dcp)) == sp.n_strengths
         ref_tab = sb.CdefDecideParams()
         orc.orc_cdef_decide_table(pick, C.byref(ref_tab))
         assert list(dcp.filter_strength) == list(ref_tab.filter_strength)
         dcp.mi_rows, dcp.mi_cols, dcp.lambda_ = mi_rows, mi_cols, 3500
-        nfb = ((mi_rows + 15) // 16) * ((mi_cols + 15) // 16)
+        self.nfb = nfb = ((mi_rows + 15) // 16) * ((mi_cols + 15) // 16)
         want_mse = np.zeros((2, nfb, 64), np.uint64)
-        pres, ss = pre.struct(), src.struct()
-        orc.orc_cdef_search(C.byref(sp), C.byref(pres), C.byref(ss), cm.ptr(skip), skip.shape[1], cm.ptr(want_mse))
-        want_dec, want_idx = sb.CdefDecision(), np.zeros(nfb, np.int8)
-        orc.orc_cdef_decide(C.byref(dcp), cm.ptr(want_mse), cm.ptr(skip), skip.shape[1], C.byref(want_dec), cm.ptr(want_idx))
+        pres, ss = pre.struct(), self.src.struct()
+        orc.orc_cdef_search(C.byref(sp), C.byref(pres), C.byref(ss), cm.ptr(self.skip), self.skip.shape[1], cm.ptr(want_mse))
+        self.want_dec, self.want_idx = sb.CdefDecision(), np.zeros(nfb, np.int8)
+        orc.orc_cdef_decide(C.byref(dcp), cm.ptr(want_mse), cm.ptr(self.skip), self.skip.shape[1], C.byref(self.want_dec), cm.ptr(self.want_idx))
         pa = sb.CdefApplyParams()
         pa.mi_rows, pa.mi_cols, pa.damping = mi_rows, mi_cols, 5
         for i in range(8):
-            pa.y_strength[i], pa.uv_strength[i] = want_dec.y_strength[i], want_dec.uv_strength[i]
-        want = pre.copy()
-        ws = want.struct()
-        orc.orc_cdef_apply(C.byref(pa), C.byref(pres), C.byref(ws), cm.ptr(skip), skip.shape[1], cm.ptr(want_idx))
-        got, gs_dec, g_idx = rec.copy(), sb.CdefDecision(), np.full(nfb, 99, np.int8)
-        gs = got.struct()
-        sb.check(lib.svt_b200_engine_dlf_cdef_frame_dev(e, C.byref(dp) if dp else None, flat, C.byref(sp), C.byref(dcp), 5, 1, C.byref(gs), C.byref(ss),
-                                                        cm.ptr(skip), skip.shape[1], C.byref(gs_dec), cm.ptr(g_idx)), lib)
-        assert (gs_dec.cdef_bits, gs_dec.nb_cdef_strengths, gs_dec.sb_count) == (want_dec.cdef_bits, want_dec.nb_cdef_strengths, want_dec.sb_count)
-        n = want_dec.nb_cdef_strengths
-        assert list(gs_dec.y_strength)[:n] == list(want_dec.y_strength)[:n] and list(gs_dec.uv_strength)[:n] == list(want_dec.uv_strength)[:n]
-        np.testing.assert_array_equal(g_idx, want_idx)
-        assert want_idx[0] == -1 and (want_idx >= 0).any()
+            pa.y_strength[i], pa.uv_strength[i] = self.want_dec.y_strength[i], self.want_dec.uv_strength[i]
+        self.want = pre.copy()
+        ws = self.want.struct()
+        orc.orc_cdef_apply(C.byref(pa), C.byref(pres), C.byref(ws), cm.ptr(self.skip), self.skip.shape[1], cm.ptr(self.want_idx))
+
+    def run(self, lib, e, apply):
+        """One engine call on a copy of the reconstruction: (rc, picture, decision, filter-block indices)."""
+        got, dec, idx = self.rec.copy(), sb.CdefDecision(), np.full(self.nfb, 99, np.int8)
+        gs, ss = got.struct(), self.src.struct()
+        rc = lib.svt_b200_engine_dlf_cdef_frame_dev(e, C.byref(self.dp) if self.dp else None, self.flat, C.byref(self.sp), C.byref(self.dcp),
+                                                    5, apply, C.byref(gs), C.byref(ss), cm.ptr(self.skip), self.skip.shape[1],
+                                                    C.byref(dec), cm.ptr(idx))
+        return rc, got, dec, idx
+
+    def decision_matches(self, dec):
+        n = self.want_dec.nb_cdef_strengths
+        return ((dec.cdef_bits, dec.nb_cdef_strengths, dec.sb_count) == (self.want_dec.cdef_bits, n, self.want_dec.sb_count) and
+                list(dec.y_strength)[:n] == list(self.want_dec.y_strength)[:n] and
+                list(dec.uv_strength)[:n] == list(self.want_dec.uv_strength)[:n])
+
+
+# 1920x1080 10-bit: the packed pictures (6.2 MB) are staged by the split host copy.  The ids of the first four cases
+# predate the size parameter.
+@pytest.mark.parametrize("w,h,bd,with_dlf,pick", [
+    pytest.param(320, 200, 8, False, 3, id="8-False-3"), pytest.param(320, 200, 10, False, 3, id="10-False-3"),
+    pytest.param(320, 200, 10, True, 2, id="10-True-2"), pytest.param(320, 200, 8, True, 3, id="8-True-3"),
+    pytest.param(1920, 1080, 10, True, 3, id="1920x1080-10-True-3")])
+def test_engine_cdef_frame_with_device_decision(w, h, bd, with_dlf, pick):
+    """deblocking -> search -> svt_b200_cdef_decide (finish_cdef_search on the device) -> apply in ONE engine call: the
+    decision, the per-filter-block choice and the filtered picture against the oracle chain."""
+    lib = sb.load()
+    c = CdefChain(w, h, bd, with_dlf, pick)
+    e = C.c_void_p()
+    sb.check(lib.svt_b200_engine_create(0, C.byref(e)), lib)
+    try:
+        rc, got, dec, idx = c.run(lib, e, 1)
+        sb.check(rc, lib)
+        assert c.decision_matches(dec)
+        np.testing.assert_array_equal(idx, c.want_idx)
+        assert c.want_idx[0] == -1 and (c.want_idx >= 0).any()
         for i in range(3):
-            np.testing.assert_array_equal(got.plane(i), want.plane(i), err_msg=f"plane {i}")
+            np.testing.assert_array_equal(got.plane(i), c.want.plane(i), err_msg=f"plane {i}")
         # apply = 0: decision only, the host picture untouched
-        again, d2, i2 = rec.copy(), sb.CdefDecision(), np.zeros(nfb, np.int8)
-        ags = again.struct()
-        sb.check(lib.svt_b200_engine_dlf_cdef_frame_dev(e, C.byref(dp) if dp else None, flat, C.byref(sp), C.byref(dcp), 5, 0, C.byref(ags), C.byref(ss),
-                                                        cm.ptr(skip), skip.shape[1], C.byref(d2), cm.ptr(i2)), lib)
-        np.testing.assert_array_equal(i2, want_idx)
+        rc, again, dec, idx = c.run(lib, e, 0)
+        sb.check(rc, lib)
+        assert c.decision_matches(dec)
+        np.testing.assert_array_equal(idx, c.want_idx)
         for i in range(3):
-            np.testing.assert_array_equal(again.plane(i), rec.plane(i))
+            np.testing.assert_array_equal(again.plane(i), c.rec.plane(i))
     finally:
         lib.svt_b200_engine_destroy(e)
 
 
-@pytest.mark.parametrize("case", [(192, 136, 8, 1, 0, 3, (20, 24, 12, 9)), (128, 128, 10, 3, 0, 3, (40, 40, 33, 20))])
+@pytest.mark.parametrize("case", [(192, 136, 8, 1, 0, 3, (20, 24, 12, 9)), (128, 128, 10, 3, 0, 3, (40, 40, 33, 20)),
+                                  (1920, 1080, 10, 4, 0, 3, (30, 26, 18, 12))])
 def test_engine_dlf_pick_frame(case):
     """Level search + deblocking as one call: the levels equal the oracle's svt_av1_pick_filter_level, the picture equals the
     oracle's deblocking with those levels (sharpness 0)."""
@@ -224,8 +264,43 @@ def test_engine_dlf_pick_frame(case):
         lib.svt_b200_engine_destroy(e)
 
 
+def lr_boundary_lines(dblk):
+    """The deblocked lines above / below every stripe boundary as svt_av1_loop_restoration_save_boundary_lines keeps them
+    (RestorationStripeBoundaries layout).  Returns the HostLrLines array and the numpy buffers it points into."""
+    lines = (sb.HostLrLines * 3)()
+    keep = []
+    for pl in range(3):
+        ss = 1 if pl else 0
+        d = dblk.plane(pl)
+        ph, pw = d.shape
+        SH, off = 64 >> ss, 8 >> ss
+        n_stripes = (ph + off + SH - 1) // SH
+        stride = pw + 16
+        above = np.zeros((2 * n_stripes, stride), d.dtype)
+        below = np.zeros((2 * n_stripes, stride), d.dtype)
+        for s in range(n_stripes):
+            y0, y1 = max(0, s * SH - off), min((s + 1) * SH - off, ph)
+            if s > 0:
+                above[2 * s, :pw], above[2 * s + 1, :pw] = d[y0 - 2], d[y0 - 1]
+            if y1 < ph:
+                below[2 * s, :pw], below[2 * s + 1, :pw] = d[y1], d[min(y1 + 1, ph - 1)]
+        keep += [above, below]
+        lines[pl].above, lines[pl].below, lines[pl].stride = above.ctypes.data, below.ctypes.data, stride
+    return lines, keep
+
+
+def lr_frame_params(units, unit_sizes, ftypes):
+    p = sb.LrFrameParams()
+    for i in range(3):
+        p.plane[i].frame_restoration_type, p.plane[i].restoration_unit_size = ftypes[i], unit_sizes[i]
+        p.plane[i].units = C.addressof(units[i])
+    p.optimized_lr = 0
+    return p, (C.c_int32 * 3)(*[len(u) for u in units])
+
+
 @pytest.mark.parametrize("case", [(192, 136, 8, 1, (64, 32, 32), ("mix", "mix", "mix"), (3, 3, 3)),
-                                  (264, 200, 10, 3, (128, 64, 64), ("mix", "mix", "none"), (3, 3, 0))])
+                                  (264, 200, 10, 3, (128, 64, 64), ("mix", "mix", "none"), (3, 3, 0)),
+                                  (1920, 1080, 10, 5, (128, 64, 64), ("mix", "mix", "mix"), (3, 3, 3))])
 def test_engine_lr_frame_from_boundary_lines(case):
     """The restoration frame filter fed the way rest_kernel feeds it: the CDEF picture plus the two deblocked lines above /
     below every 64-row stripe (RestorationStripeBoundaries layout), not the whole deblocked picture."""
@@ -237,31 +312,8 @@ def test_engine_lr_frame_from_boundary_lines(case):
         w, h, bd, seed, unit_sizes, modes, ftypes = case
         cdef, dblk, units = lr_case(w, h, bd, seed, unit_sizes, modes)
         want = run_oracle_lr(cdef, dblk, units, unit_sizes, ftypes, 0)
-        lines = (sb.HostLrLines * 3)()
-        keep = []
-        for pl in range(3):
-            ss = 1 if pl else 0
-            d = dblk.plane(pl)
-            ph, pw = d.shape
-            SH, off = 64 >> ss, 8 >> ss
-            n_stripes = (ph + off + SH - 1) // SH
-            stride = pw + 16
-            above = np.zeros((2 * n_stripes, stride), d.dtype)
-            below = np.zeros((2 * n_stripes, stride), d.dtype)
-            for s in range(n_stripes):
-                y0, y1 = max(0, s * SH - off), min((s + 1) * SH - off, ph)
-                if s > 0:
-                    above[2 * s, :pw], above[2 * s + 1, :pw] = d[y0 - 2], d[y0 - 1]
-                if y1 < ph:
-                    below[2 * s, :pw], below[2 * s + 1, :pw] = d[y1], d[min(y1 + 1, ph - 1)]
-            keep += [above, below]
-            lines[pl].above, lines[pl].below, lines[pl].stride = above.ctypes.data, below.ctypes.data, stride
-        p = sb.LrFrameParams()
-        for i in range(3):
-            p.plane[i].frame_restoration_type, p.plane[i].restoration_unit_size = ftypes[i], unit_sizes[i]
-            p.plane[i].units = C.addressof(units[i])
-        p.optimized_lr = 0
-        n_units = (C.c_int32 * 3)(*[len(u) for u in units])
+        lines, keep = lr_boundary_lines(dblk)
+        p, n_units = lr_frame_params(units, unit_sizes, ftypes)
         got = cdef.copy()
         gs = got.struct()
         sb.check(lib.svt_b200_engine_lr_frame(e, C.byref(p), n_units, C.byref(gs), lines), lib)
