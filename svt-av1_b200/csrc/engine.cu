@@ -34,8 +34,17 @@ constexpr int kMeSlots = 8;       // concurrent ME pictures
 constexpr int kFiltSlots = 8;     // concurrent deblock / CDEF pictures
 constexpr int kPlaneEntries = 96; // resident ME pictures (3.3 MB each at 1080p, 13 MB at 2160p); >= kMeSlots * 9 so that
                                   // every in-flight picture can hold its source + 8 references at once (no deadlock)
+constexpr size_t kLutBytes = 3 * 2 * 128; // the level table of svt_b200_lf_level_lut
 
 inline size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// The next piece of an arena: pieces start 256-byte aligned, in the order they are taken.
+template <typename T = uint8_t>
+T *carve(uint8_t *&p, size_t bytes) {
+    T *r = reinterpret_cast<T *>(p);
+    p += al256(bytes);
+    return r;
+}
 
 struct PlaneEntry {
     const void *key = nullptr;
@@ -53,32 +62,45 @@ struct MeSlot {
     cudaEvent_t up_done = nullptr; // the staging buffer has been consumed by its upload
     bool up_pending = false;
     uint8_t *scratch = nullptr;
-    uint8_t *dev = nullptr;     // best_sad | best_mv | hme | me_mv | me_cand | total | rc
+    SvtB200MeOutputs out = {};  // device; me_mv | me_cand | total_cand | rc_me_distortion are contiguous
     uint8_t *pin_up = nullptr;  // full | quarter | sixteenth of one picture
-    uint8_t *pin_out = nullptr; // me_mv | me_cand | total | rc
+    int16_t *pin_mv = nullptr;  // pinned copies of the four contiguous outputs, laid out alike: one read-back
+    uint8_t *pin_cand = nullptr, *pin_tot = nullptr;
+    uint32_t *pin_rc = nullptr;
 };
 
 struct FiltSlot {
     bool busy = false;
     cudaStream_t st = nullptr;
     SvtB200Frame recon, out, source; // device pictures
-    uint8_t *misc = nullptr;         // mi array | skip8 | mse | fb idx
-    uint8_t *pin_a = nullptr;        // packed picture (reconstruction up / down)
-    uint8_t *pin_b = nullptr;        // packed picture (source); the mode-info array for deblocking
-    uint8_t *pin_small = nullptr;    // skip map | mse | fb idx | decision
-    uint8_t *pin_mi = nullptr;       // the mode-info array when the call must not reuse pin_b (single-sync path)
+    // device, in this order: the LR units take the whole region from `mi` on
+    SvtB200DlfMi *mi = nullptr;
+    uint8_t *pick = nullptr; // svt_b200_pick_filter_level's scratch
+    uint8_t *lut = nullptr;  // the level table of the picked levels
+    uint8_t *skip = nullptr;
+    uint64_t *mse = nullptr;
+    int8_t *idx = nullptr;                 // filter-block strength indices,
+    SvtB200CdefDecision *dec = nullptr;    // then the decision: one read-back
+    uint8_t *decide = nullptr;             // svt_b200_cdef_decide's scratch
+    // pinned
+    uint8_t *pin_a = nullptr;     // packed picture (reconstruction up / down)
+    uint8_t *pin_b = nullptr;     // packed picture (source), or the LR boundary lines
+    uint8_t *pin_small = nullptr; // skip map | mse | fb idx | decision; also stages the LR units and the level table
+    int8_t *pin_idx = nullptr;
+    SvtB200CdefDecision *pin_dec = nullptr;
+    SvtB200DlfMi *pin_mi = nullptr; // the mode-info array
 };
 
 struct MeGeom {
     size_t nb[3] = {0, 0, 0}, entry = 0, n_sb = 0, scratch = 0;
-    size_t b_sad = 0, b_hme = 0, b_mv = 0, b_cand = 0, b_tot = 0, b_rc = 0, o_mv = 0, o_cand = 0, o_tot = 0, o_rc = 0, dev = 0, out = 0;
+    size_t b_sad = 0, b_hme = 0, b_mv = 0, b_cand = 0, b_tot = 0, b_rc = 0, dev = 0, out = 0;
     bool operator==(const MeGeom &o) const { return nb[0] == o.nb[0] && nb[1] == o.nb[1] && nb[2] == o.nb[2] && n_sb == o.n_sb; }
 };
 
 struct FiltGeom {
     int w = 0, h = 0, bd = 0, mi_rows = 0, mi_cols = 0;
     int sy = 0, sc = 0; // device strides (samples)
-    size_t by = 0, bc = 0, frame = 0, packed = 0, mi = 0, skip = 0, mse = 0, nfb = 0, misc = 0, small = 0, idx = 0, dec = 0;
+    size_t by = 0, bc = 0, frame = 0, packed = 0, mi = 0, skip = 0, mse = 0, nfb = 0, misc = 0, small = 0, idx = 0, decide = 0;
     bool same(int w_, int h_, int bd_) const { return w == w_ && h == h_ && bd == bd_; }
 };
 
@@ -118,13 +140,19 @@ struct Lap { // accumulates wall time into an engine counter
     ~Lap() { acc += now_ns() - t0; }
 };
 
+// ENG_TRY(expr): return from the calling function when expr fails.  expr is either a CUDA runtime call, whose error
+// becomes the thread's message here, or a status from the library's entries and the engine's helpers, which set their
+// own message.
+inline int eng_status(cudaError_t err, const char *expr, const char *file, int line) {
+    if (err == cudaSuccess) return SVT_B200_OK;
+    set_error("engine: %s failed: %s (%s:%d)", expr, cudaGetErrorString(err), file, line);
+    return SVT_B200_ERR_CUDA;
+}
+inline int eng_status(int rc, const char *, const char *, int) { return rc; }
 #define ENG_TRY(expr)                                                                                              \
     do {                                                                                                           \
-        cudaError_t e__ = (expr);                                                                                  \
-        if (e__ != cudaSuccess) {                                                                                  \
-            set_error("engine: %s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__);        \
-            return SVT_B200_ERR_CUDA;                                                                              \
-        }                                                                                                          \
+        const int rc__ = eng_status((expr), #expr, __FILE__, __LINE__);                                            \
+        if (rc__ != SVT_B200_OK) return rc__;                                                                      \
     } while (0)
 
 template <typename Slot, int N>
@@ -140,14 +168,6 @@ Slot *acquire(SvtB200Engine *e, Slot (&pool)[N]) {
         e->cv.wait(lk);
     }
 }
-template <typename Slot>
-void release(SvtB200Engine *e, Slot *s) {
-    {
-        std::lock_guard<std::mutex> g(e->mu);
-        s->busy = false;
-    }
-    e->cv.notify_all();
-}
 
 cudaError_t timed_sync(SvtB200Engine *e, cudaStream_t st) {
     Lap lap(e->stats.ns_sync);
@@ -155,6 +175,20 @@ cudaError_t timed_sync(SvtB200Engine *e, cudaStream_t st) {
 }
 
 size_t plane_bytes(const SvtB200Plane &g) { return (size_t)g.stride * (size_t)(g.height + 2 * g.origin_y); }
+
+// The device arena and the pinned arena of one side: both or, after a failure, neither.
+int alloc_arenas(SvtB200Engine *e, uint8_t **dev, size_t dev_bytes, uint8_t **pin, size_t pin_bytes) {
+    ENG_TRY(cudaMalloc((void **)dev, dev_bytes));
+    const cudaError_t err = cudaMallocHost((void **)pin, pin_bytes);
+    if (err != cudaSuccess) {
+        cudaFree(*dev);
+        *dev = nullptr;
+        set_error("engine: cudaMallocHost of %zu bytes failed: %s", pin_bytes, cudaGetErrorString(err));
+        return SVT_B200_ERR_CUDA;
+    }
+    e->stats.pinned_bytes += pin_bytes;
+    return SVT_B200_OK;
+}
 
 // ---- one-time allocation for the ME side --------------------------------------------------------------------------
 int ensure_me(SvtB200Engine *e, const SvtB200MeParams *p) {
@@ -177,31 +211,28 @@ int ensure_me(SvtB200Engine *e, const SvtB200MeParams *p) {
     g.b_cand = g.n_sb * 85 * 23;
     g.b_tot = g.n_sb * 85;
     g.b_rc = g.n_sb * 4;
-    g.o_mv = 2 * al256(g.b_sad) + al256(g.b_hme);
-    g.o_cand = g.o_mv + al256(g.b_mv);
-    g.o_tot = g.o_cand + al256(g.b_cand);
-    g.o_rc = g.o_tot + al256(g.b_tot);
-    g.dev = g.o_rc + al256(g.b_rc);
-    g.out = g.dev - g.o_mv;
+    g.out = al256(g.b_mv) + al256(g.b_cand) + al256(g.b_tot) + al256(g.b_rc);
+    g.dev = 2 * al256(g.b_sad) + al256(g.b_hme) + g.out;
     const size_t dev_total = (size_t)kPlaneEntries * g.entry + (size_t)kMeSlots * (g.scratch + g.dev);
-    const size_t pin_total = (size_t)kMeSlots * (g.entry + al256(g.out));
-    ENG_TRY(cudaMalloc((void **)&e->me_dev, dev_total));
-    ENG_TRY(cudaMallocHost((void **)&e->me_pin, pin_total));
-    e->stats.pinned_bytes += pin_total;
+    const size_t pin_total = (size_t)kMeSlots * (g.entry + g.out);
+    ENG_TRY(alloc_arenas(e, &e->me_dev, dev_total, &e->me_pin, pin_total));
     uint8_t *d = e->me_dev, *h = e->me_pin;
-    for (auto &c : e->planes) {
-        c.d[0] = d;
-        c.d[1] = d + al256(g.nb[0]);
-        c.d[2] = c.d[1] + al256(g.nb[1]);
-        d += g.entry;
-    }
+    for (auto &c : e->planes)
+        for (int i = 0; i < 3; i++) c.d[i] = carve(d, g.nb[i]);
     for (auto &s : e->me) {
-        s.scratch = d;
-        s.dev = d + g.scratch;
-        d += g.scratch + g.dev;
-        s.pin_up = h;
-        s.pin_out = h + g.entry;
-        h += g.entry + al256(g.out);
+        s.scratch = carve(d, g.scratch);
+        s.out.best_sad = carve<uint32_t>(d, g.b_sad);
+        s.out.best_mv = carve<uint32_t>(d, g.b_sad);
+        s.out.hme = carve<SvtB200HmeResult>(d, g.b_hme);
+        s.out.me_mv = carve<int16_t>(d, g.b_mv);
+        s.out.me_cand = carve(d, g.b_cand);
+        s.out.total_cand = carve(d, g.b_tot);
+        s.out.rc_me_distortion = carve<uint32_t>(d, g.b_rc);
+        s.pin_up = carve(h, g.entry);
+        s.pin_mv = carve<int16_t>(h, g.b_mv);
+        s.pin_cand = carve(h, g.b_cand);
+        s.pin_tot = carve(h, g.b_tot);
+        s.pin_rc = carve<uint32_t>(h, g.b_rc);
     }
     e->mg = g;
     e->me_ready = true;
@@ -230,36 +261,39 @@ int ensure_filt(SvtB200Engine *e, int w, int h, int bd, int mi_rows, int mi_cols
     g.skip = al256((size_t)((mi_rows + 1) / 2) * ((((mi_cols + 1) / 2) + 15) & ~15));
     g.mse = al256(g.nfb * 2 * 64 * 8);
     g.idx = al256(g.nfb);
-    g.dec = al256(sizeof(SvtB200CdefDecision)) + al256(g.nfb * (16 + 16 * 64) + 64); // the device decision + cdef_decide's scratch (any table size)
-    g.small = g.skip + g.mse + g.idx + g.dec;
-    g.misc = g.mi + 4096 + g.small; // mode-info summary | the level search's scratch | skip map, mse, filter-block indices
+    g.decide = al256(g.nfb * (16 + 16 * 64) + 64); // any table size
+    g.small = g.skip + g.mse + g.idx + al256(sizeof(SvtB200CdefDecision)) + g.decide;
+    g.misc = g.mi + 4096 + g.small; // mode-info array | the level search's scratch and table | skip map ... decide scratch
     const size_t dev_total = (size_t)kFiltSlots * (3 * g.frame + g.misc);
-    const size_t pin_b = std::max(g.packed, g.mi);
-    const size_t pin_total = (size_t)kFiltSlots * (g.packed + pin_b + g.small + g.mi);
-    ENG_TRY(cudaMalloc((void **)&e->filt_dev, dev_total));
-    ENG_TRY(cudaMallocHost((void **)&e->filt_pin, pin_total));
-    e->stats.pinned_bytes += pin_total;
+    const size_t pin_total = (size_t)kFiltSlots * (2 * g.packed + g.small + g.mi);
+    ENG_TRY(alloc_arenas(e, &e->filt_dev, dev_total, &e->filt_pin, pin_total));
     uint8_t *d = e->filt_dev, *hp = e->filt_pin;
     for (auto &s : e->filt) {
-        SvtB200Frame *fr[3] = {&s.recon, &s.out, &s.source};
-        for (SvtB200Frame *f : fr) {
-            f->y = d + 512; // margin: the filters' vector loads may touch a few bytes before sample (0,0)
-            f->cb = d + 512 + g.by;
-            f->cr = d + 512 + g.by + g.bc;
+        for (SvtB200Frame *f : {&s.recon, &s.out, &s.source}) {
+            uint8_t *b = carve(d, g.frame) + 512; // margin: the filters' vector loads may touch a few bytes before sample (0,0)
+            f->y = b;
+            f->cb = b + g.by;
+            f->cr = b + g.by + g.bc;
             f->stride_y = g.sy;
             f->stride_c = g.sc;
             f->width = w;
             f->height = h;
             f->bit_depth = bd;
-            d += g.frame;
         }
-        s.misc = d;
-        d += g.misc;
-        s.pin_a = hp;
-        s.pin_b = hp + g.packed;
-        s.pin_small = s.pin_b + pin_b;
-        s.pin_mi = s.pin_small + g.small;
-        hp += g.packed + pin_b + g.small + g.mi;
+        s.mi = carve<SvtB200DlfMi>(d, g.mi);
+        s.pick = carve(d, 1024);
+        s.lut = carve(d, 4096 - 1024);
+        s.skip = carve(d, g.skip);
+        s.mse = carve<uint64_t>(d, g.mse);
+        s.idx = carve<int8_t>(d, g.idx);
+        s.dec = carve<SvtB200CdefDecision>(d, sizeof(SvtB200CdefDecision));
+        s.decide = carve(d, g.decide);
+        s.pin_a = carve(hp, g.packed);
+        s.pin_b = carve(hp, g.packed);
+        s.pin_small = carve(hp, g.skip + g.mse); // the host uses neither the mse nor the decide-scratch part
+        s.pin_idx = carve<int8_t>(hp, g.idx);
+        s.pin_dec = carve<SvtB200CdefDecision>(hp, al256(sizeof(SvtB200CdefDecision)) + g.decide);
+        s.pin_mi = carve<SvtB200DlfMi>(hp, g.mi);
     }
     e->fg = g;
     e->filt_ready = true;
@@ -288,10 +322,96 @@ void par_memcpy(void *dst, const void *src, size_t n) {
     for (auto &t : th) t.join();
 }
 
-// Make the three planes of `pic` resident and ordered before later work on the slot's stream.  users++ on return.
-int plane_acquire(SvtB200Engine *e, MeSlot *s, const SvtB200MeParams *p, const SvtB200HostMePicture *pic, int filtered_ds,
-                  PlaneEntry **out) {
+// Every copy between pinned staging and the device goes through these two, which count the bytes they move.
+void count_bytes(SvtB200Engine *e, cudaMemcpyKind kind, size_t n) {
+    (kind == cudaMemcpyHostToDevice ? e->stats.h2d_bytes : e->stats.d2h_bytes) += n;
+}
+int copy_async(SvtB200Engine *e, void *dst, const void *src, size_t n, cudaMemcpyKind kind, cudaStream_t st) {
+    ENG_TRY(cudaMemcpyAsync(dst, src, n, kind, st));
+    count_bytes(e, kind, n);
+    return SVT_B200_OK;
+}
+int copy_2d_async(SvtB200Engine *e, void *dst, size_t dpitch, const void *src, size_t spitch, size_t row, size_t rows,
+                  cudaMemcpyKind kind, cudaStream_t st) {
+    ENG_TRY(cudaMemcpy2DAsync(dst, dpitch, src, spitch, row, rows, kind, st));
+    count_bytes(e, kind, row * rows);
+    return SVT_B200_OK;
+}
+
+// The loader's part of plane_acquire: stage `pic` and upload it to `en` on the slot's stream (only the full plane when
+// the decimations are derived on the device), then record `en`'s ready event.
+int load_planes(SvtB200Engine *e, MeSlot *s, const SvtB200MeParams *p, const SvtB200HostMePicture *pic, int filtered_ds,
+                PlaneEntry *en) {
     const MeGeom &g = e->mg;
+    const bool gen = !pic->quarter || !pic->sixteenth; // decimations derived on the device
+    if (s->up_pending) { // the staging buffer still feeds the previous upload of this call
+        s->up_pending = false;
+        ENG_TRY(cudaEventSynchronize(s->up_done));
+    }
+    size_t bytes = g.nb[0];
+    {
+        Lap lap(e->stats.ns_host_copy);
+        par_memcpy(s->pin_up, pic->full, g.nb[0]);
+        if (!gen) {
+            memcpy(s->pin_up + al256(g.nb[0]), pic->quarter, g.nb[1]);
+            memcpy(s->pin_up + al256(g.nb[0]) + al256(g.nb[1]), pic->sixteenth, g.nb[2]);
+            bytes = al256(g.nb[0]) + al256(g.nb[1]) + g.nb[2]; // the three planes are laid out alike on both sides
+        }
+    }
+    ENG_TRY(copy_async(e, en->d[0], s->pin_up, bytes, cudaMemcpyHostToDevice, s->st));
+    ENG_TRY(cudaEventRecord(s->up_done, s->st));
+    s->up_pending = true;
+    if (gen) {
+        const SvtB200MePlanes dp = {en->d[0], en->d[1], en->d[2]};
+        ENG_TRY(svt_b200_me_downsample(&p->full, &p->quarter, &p->sixteenth, &dp, filtered_ds, s->st));
+    }
+    ENG_TRY(cudaEventRecord(en->ready, s->st));
+    return SVT_B200_OK;
+}
+
+// A filter slot for the scope of one call.  A call that returns before its final stream wait may have left work on the
+// slot's stream: the destructor waits for it before the slot can serve another call.
+struct FiltLease {
+    SvtB200Engine *e;
+    FiltSlot *s;
+    bool done = false; // the call's stream wait succeeded
+    explicit FiltLease(SvtB200Engine *e_) : e(e_), s(acquire(e_, e_->filt)) {}
+    ~FiltLease() {
+        if (!done) cudaStreamSynchronize(s->st);
+        {
+            std::lock_guard<std::mutex> g(e->mu);
+            s->busy = false;
+        }
+        e->cv.notify_all();
+    }
+};
+
+// An ME slot and the plane entries its call made resident, for the scope of one call.  The entries are released after
+// the stream wait: nothing of the picture may still read a plane when its entry is handed back.
+struct MeLease {
+    SvtB200Engine *e;
+    MeSlot *s;
+    PlaneEntry *ents[1 + SVT_B200_ME_LISTS * SVT_B200_ME_MAX_REFS] = {};
+    int n_ent = 0;
+    bool done = false; // the call's stream wait succeeded
+    explicit MeLease(SvtB200Engine *e_) : e(e_), s(acquire(e_, e_->me)) {}
+    ~MeLease() {
+        if (!done) cudaStreamSynchronize(s->st);
+        s->up_pending = false;
+        {
+            std::lock_guard<std::mutex> g(e->mu);
+            for (int i = 0; i < n_ent; i++) ents[i]->users--;
+            s->busy = false;
+        }
+        e->cv.notify_all();
+    }
+};
+
+// Make the three planes of `pic` resident and ordered before later work on the slot's stream.  The lease holds the
+// entry until it ends.
+int plane_acquire(SvtB200Engine *e, MeLease &L, const SvtB200MeParams *p, const SvtB200HostMePicture *pic, int filtered_ds,
+                  SvtB200MePlanes *out) {
+    MeSlot *s = L.s;
     PlaneEntry *en = nullptr;
     bool loader = false;
     {
@@ -336,62 +456,46 @@ int plane_acquire(SvtB200Engine *e, MeSlot *s, const SvtB200MeParams *p, const S
         en->stamp = ++e->clock;
     }
     if (loader) {
-        int rc = SVT_B200_OK;
-        const bool gen = !pic->quarter || !pic->sixteenth; // decimations derived on the device
-        if (s->up_pending) { // the staging buffer still feeds the previous upload of this call
-            if (cudaEventSynchronize(s->up_done) != cudaSuccess) rc = SVT_B200_ERR_CUDA;
-            s->up_pending = false;
-        }
-        size_t bytes = 0;
-        if (rc == SVT_B200_OK) {
-            Lap lap(e->stats.ns_host_copy);
-            par_memcpy(s->pin_up, pic->full, g.nb[0]);
-            bytes = g.nb[0];
-            if (!gen) {
-                memcpy(s->pin_up + al256(g.nb[0]), pic->quarter, g.nb[1]);
-                memcpy(s->pin_up + al256(g.nb[0]) + al256(g.nb[1]), pic->sixteenth, g.nb[2]);
-                bytes = al256(g.nb[0]) + al256(g.nb[1]) + g.nb[2]; // the three planes are laid out alike on both sides
-            }
-        }
-        if (rc == SVT_B200_OK && cudaMemcpyAsync(en->d[0], s->pin_up, bytes, cudaMemcpyHostToDevice, s->st) != cudaSuccess)
-            rc = SVT_B200_ERR_CUDA;
-        if (rc == SVT_B200_OK && cudaEventRecord(s->up_done, s->st) != cudaSuccess) rc = SVT_B200_ERR_CUDA;
-        s->up_pending = rc == SVT_B200_OK;
-        e->stats.h2d_bytes += bytes;
-        if (rc == SVT_B200_OK && gen) {
-            SvtB200MePlanes dp = {en->d[0], en->d[1], en->d[2]};
-            rc = svt_b200_me_downsample(&p->full, &p->quarter, &p->sixteenth, &dp, filtered_ds, s->st);
-        }
-        if (rc == SVT_B200_OK && cudaEventRecord(en->ready, s->st) != cudaSuccess) rc = SVT_B200_ERR_CUDA;
+        const int rc = load_planes(e, s, p, pic, filtered_ds, en);
         {
             std::lock_guard<std::mutex> gl(e->mu);
             en->state = rc == SVT_B200_OK ? 2 : 0;
             if (rc != SVT_B200_OK) en->users--;
         }
         e->cv.notify_all();
-        if (rc != SVT_B200_OK) {
-            if (rc == SVT_B200_ERR_CUDA) set_error("engine: ME plane upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-            return rc;
-        }
-    } else {
-        ENG_TRY(cudaStreamWaitEvent(s->st, en->ready, 0));
+        if (rc != SVT_B200_OK) return rc;
     }
-    *out = en;
+    L.ents[L.n_ent++] = en;
+    if (!loader) ENG_TRY(cudaStreamWaitEvent(s->st, en->ready, 0));
+    *out = {en->d[0], en->d[1], en->d[2]};
     return SVT_B200_OK;
 }
 
-void plane_release(SvtB200Engine *e, PlaneEntry **ents, int n) {
-    {
-        std::lock_guard<std::mutex> g(e->mu);
-        for (int i = 0; i < n; i++)
-            if (ents[i]) ents[i]->users--;
+// The packed layout of a picture in pinned staging: tight rows, planes y, cb, cr one after another.  The host copies
+// and the DMA copies of a picture both take it from here.
+struct Packed {
+    int bps = 0;              // bytes per sample
+    int w[3], h[3];           // plane sizes in samples
+    size_t row[3], off[3];    // bytes per packed row; where each plane starts in the staging buffer
+    uint8_t *plane[3];        // the picture's planes
+    size_t pitch[3];          // the picture's row pitches in bytes
+    size_t bytes = 0;         // the whole packed picture
+    explicit Packed(const SvtB200Frame *f) : bps(f->bit_depth > 8 ? 2 : 1) {
+        for (int i = 0; i < 3; i++) {
+            w[i] = i ? (f->width + 1) >> 1 : f->width;
+            h[i] = i ? (f->height + 1) >> 1 : f->height;
+            row[i] = (size_t)w[i] * bps;
+            off[i] = bytes;
+            bytes += row[i] * h[i];
+            plane[i] = (uint8_t *)(i == 0 ? f->y : i == 1 ? f->cb : f->cr);
+            pitch[i] = (size_t)(i ? f->stride_c : f->stride_y) * bps;
+        }
     }
-    e->cv.notify_all();
-}
+};
 
-// host picture <-> packed (tight rows: y, cb, cr) pinned staging.  A 2160p 10-bit picture is 25 MB and one pipeline
-// thread copies only a few GB/s (the picture pools of the encoder may be spread over both sockets of the host), so
-// pictures above 4 MB are split by rows over four threads.
+// host picture <-> packed pinned staging.  A 2160p 10-bit picture is 25 MB and one pipeline thread copies only a few
+// GB/s (the picture pools of the encoder may be spread over both sockets of the host), so pictures above 4 MB are split
+// by rows over four threads.
 struct RowCopy {
     uint8_t *dst;
     const uint8_t *src;
@@ -418,37 +522,28 @@ void run_copies(SvtB200Engine *e, const RowCopy (&c)[3]) {
     part(0);
     for (int t = 1; t < nt; t++) th[t - 1].join();
 }
-void pack_frame(SvtB200Engine *e, uint8_t *pin, const SvtB200Frame *h) {
-    const int bps = h->bit_depth > 8 ? 2 : 1, cw = (h->width + 1) >> 1, ch = (h->height + 1) >> 1;
-    const size_t rw = (size_t)h->width * bps, rc = (size_t)cw * bps;
-    const RowCopy c[3] = {{pin, (const uint8_t *)h->y, rw, (size_t)h->stride_y * bps, rw, h->height},
-                          {pin + rw * h->height, (const uint8_t *)h->cb, rc, (size_t)h->stride_c * bps, rc, ch},
-                          {pin + rw * h->height + rc * ch, (const uint8_t *)h->cr, rc, (size_t)h->stride_c * bps, rc, ch}};
+void pack_frame(SvtB200Engine *e, uint8_t *pin, const SvtB200Frame *f) {
+    const Packed k(f);
+    RowCopy c[3];
+    for (int i = 0; i < 3; i++) c[i] = {pin + k.off[i], k.plane[i], k.row[i], k.pitch[i], k.row[i], k.h[i]};
     run_copies(e, c);
 }
-void unpack_frame(SvtB200Engine *e, const SvtB200Frame *h, const uint8_t *pin) {
-    const int bps = h->bit_depth > 8 ? 2 : 1, cw = (h->width + 1) >> 1, ch = (h->height + 1) >> 1;
-    const size_t rw = (size_t)h->width * bps, rc = (size_t)cw * bps;
-    const RowCopy c[3] = {{(uint8_t *)h->y, pin, (size_t)h->stride_y * bps, rw, rw, h->height},
-                          {(uint8_t *)h->cb, pin + rw * h->height, (size_t)h->stride_c * bps, rc, rc, ch},
-                          {(uint8_t *)h->cr, pin + rw * h->height + rc * ch, (size_t)h->stride_c * bps, rc, rc, ch}};
+// planes: bit i set = write plane i of `f`
+void unpack_frame(SvtB200Engine *e, const SvtB200Frame *f, const uint8_t *pin, unsigned planes = 7) {
+    const Packed k(f);
+    RowCopy c[3] = {};
+    for (int i = 0; i < 3; i++)
+        if (planes >> i & 1) c[i] = {k.plane[i], pin + k.off[i], k.pitch[i], k.row[i], k.row[i], k.h[i]};
     run_copies(e, c);
 }
 // packed pinned staging <-> device picture (three 2-D copies; both sides page-locked / device: pure DMA, asynchronous)
 int copy_packed(SvtB200Engine *e, const SvtB200Frame *dev, uint8_t *pin, cudaMemcpyKind kind, cudaStream_t st) {
-    const int bps = dev->bit_depth > 8 ? 2 : 1, cw = (dev->width + 1) >> 1, ch = (dev->height + 1) >> 1;
-    const size_t rw = (size_t)dev->width * bps, rc = (size_t)cw * bps;
-    uint8_t *py = pin, *pcb = pin + rw * dev->height, *pcr = pcb + rc * ch;
-    if (kind == cudaMemcpyHostToDevice) {
-        ENG_TRY(cudaMemcpy2DAsync(dev->y, (size_t)dev->stride_y * bps, py, rw, rw, dev->height, kind, st));
-        ENG_TRY(cudaMemcpy2DAsync(dev->cb, (size_t)dev->stride_c * bps, pcb, rc, rc, ch, kind, st));
-        ENG_TRY(cudaMemcpy2DAsync(dev->cr, (size_t)dev->stride_c * bps, pcr, rc, rc, ch, kind, st));
-        e->stats.h2d_bytes += rw * dev->height + 2 * rc * ch;
-    } else {
-        ENG_TRY(cudaMemcpy2DAsync(py, rw, dev->y, (size_t)dev->stride_y * bps, rw, dev->height, kind, st));
-        ENG_TRY(cudaMemcpy2DAsync(pcb, rc, dev->cb, (size_t)dev->stride_c * bps, rc, ch, kind, st));
-        ENG_TRY(cudaMemcpy2DAsync(pcr, rc, dev->cr, (size_t)dev->stride_c * bps, rc, ch, kind, st));
-        e->stats.d2h_bytes += rw * dev->height + 2 * rc * ch;
+    const Packed k(dev);
+    const bool up = kind == cudaMemcpyHostToDevice;
+    for (int i = 0; i < 3; i++) {
+        uint8_t *p = pin + k.off[i];
+        ENG_TRY(copy_2d_async(e, up ? k.plane[i] : p, up ? k.pitch[i] : k.row[i], up ? p : k.plane[i], up ? k.row[i] : k.pitch[i],
+                              k.row[i], k.h[i], kind, st));
     }
     return SVT_B200_OK;
 }
@@ -467,6 +562,17 @@ struct DeviceGuard { // engine calls come from arbitrary pipeline threads: bind 
     }
 };
 
+int create_streams(SvtB200Engine *e) {
+    DeviceGuard g(e->device);
+    for (auto &s : e->me) {
+        ENG_TRY(cudaStreamCreateWithFlags(&s.st, cudaStreamNonBlocking));
+        ENG_TRY(cudaEventCreateWithFlags(&s.up_done, cudaEventDisableTiming));
+    }
+    for (auto &s : e->filt) ENG_TRY(cudaStreamCreateWithFlags(&s.st, cudaStreamNonBlocking));
+    for (auto &c : e->planes) ENG_TRY(cudaEventCreateWithFlags(&c.ready, cudaEventDisableTiming));
+    return SVT_B200_OK;
+}
+
 } // namespace
 
 extern "C" {
@@ -480,13 +586,10 @@ int svt_b200_engine_create(int device, SvtB200Engine **out) {
     }
     SvtB200Engine *e = new SvtB200Engine();
     e->device = device;
-    DeviceGuard g(device);
-    for (auto &s : e->me) {
-        ENG_TRY(cudaStreamCreateWithFlags(&s.st, cudaStreamNonBlocking));
-        ENG_TRY(cudaEventCreateWithFlags(&s.up_done, cudaEventDisableTiming));
+    if (const int rc = create_streams(e)) {
+        svt_b200_engine_destroy(e);
+        return rc;
     }
-    for (auto &s : e->filt) ENG_TRY(cudaStreamCreateWithFlags(&s.st, cudaStreamNonBlocking));
-    for (auto &c : e->planes) ENG_TRY(cudaEventCreateWithFlags(&c.ready, cudaEventDisableTiming));
     *out = e;
     return SVT_B200_OK;
 }
@@ -538,70 +641,40 @@ int svt_b200_engine_me_picture(SvtB200Engine *e, const SvtB200MeParams *p, const
         set_error("svt_b200_engine_me_picture: null argument");
         return SVT_B200_ERR_ARG;
     }
-    DeviceGuard dg(e->device);
-    int rc = ensure_me(e, p);
-    if (rc != SVT_B200_OK) return rc;
-    const MeGeom &g = e->mg;
-    MeSlot *s = acquire(e, e->me);
-    PlaneEntry *ents[1 + SVT_B200_ME_LISTS * SVT_B200_ME_MAX_REFS] = {nullptr};
-    int n_ent = 0;
-    do {
-        SvtB200MePlanes dsrc, drefs[SVT_B200_ME_LISTS][SVT_B200_ME_MAX_REFS];
-        memset(drefs, 0, sizeof(drefs));
-        {
-            Lap lap(e->stats.ns_issue);
-            if ((rc = plane_acquire(e, s, p, src, filtered_downsample, &ents[n_ent])) != SVT_B200_OK) break;
-            dsrc = {ents[n_ent]->d[0], ents[n_ent]->d[1], ents[n_ent]->d[2]};
-            n_ent++;
-            for (int l = 0; l < p->num_lists && rc == SVT_B200_OK; l++)
-                for (int r = 0; r < p->num_refs[l] && rc == SVT_B200_OK; r++) {
-                    if (!refs[l][r].full) {
-                        set_error("svt_b200_engine_me_picture: reference [%d][%d] has no planes", l, r);
-                        rc = SVT_B200_ERR_ARG;
-                        break;
-                    }
-                    if ((rc = plane_acquire(e, s, p, &refs[l][r], filtered_downsample, &ents[n_ent])) != SVT_B200_OK) break;
-                    drefs[l][r] = {ents[n_ent]->d[0], ents[n_ent]->d[1], ents[n_ent]->d[2]};
-                    n_ent++;
-                }
-            if (rc != SVT_B200_OK) break;
-            SvtB200MeOutputs o;
-            o.best_sad = (uint32_t *)s->dev;
-            o.best_mv = (uint32_t *)(s->dev + al256(g.b_sad));
-            o.hme = (SvtB200HmeResult *)(s->dev + 2 * al256(g.b_sad));
-            o.me_mv = (int16_t *)(s->dev + g.o_mv);
-            o.me_cand = s->dev + g.o_cand;
-            o.total_cand = s->dev + g.o_tot;
-            o.rc_me_distortion = (uint32_t *)(s->dev + g.o_rc);
-            if ((rc = svt_b200_me_picture(p, &dsrc, drefs, &o, s->scratch, s->st)) != SVT_B200_OK) break;
-            // the four result arrays are contiguous on the device: one read-back
-            if (cudaMemcpyAsync(s->pin_out, s->dev + g.o_mv, g.out, cudaMemcpyDeviceToHost, s->st) != cudaSuccess) {
-                set_error("engine: ME read-back failed: %s", cudaGetErrorString(cudaGetLastError()));
-                rc = SVT_B200_ERR_CUDA;
-                break;
+    for (int l = 0; l < p->num_lists; l++) {
+        if (l >= SVT_B200_ME_LISTS || p->num_refs[l] > SVT_B200_ME_MAX_REFS) {
+            set_error("svt_b200_engine_me_picture: more reference lists or references than SvtB200MeParams holds");
+            return SVT_B200_ERR_ARG;
+        }
+        for (int r = 0; r < p->num_refs[l]; r++)
+            if (!refs[l][r].full) {
+                set_error("svt_b200_engine_me_picture: reference [%d][%d] has no planes", l, r);
+                return SVT_B200_ERR_ARG;
             }
-        }
-        if (timed_sync(e, s->st) != cudaSuccess) {
-            set_error("engine: ME failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = SVT_B200_ERR_CUDA;
-            break;
-        }
-        s->up_pending = false;
-        Lap lap(e->stats.ns_host_copy);
-        memcpy(me_mv, s->pin_out, g.b_mv);
-        memcpy(me_cand, s->pin_out + (g.o_cand - g.o_mv), g.b_cand);
-        memcpy(total_cand, s->pin_out + (g.o_tot - g.o_mv), g.b_tot);
-        memcpy(rc_me_distortion, s->pin_out + (g.o_rc - g.o_mv), g.b_rc);
-        e->stats.me_pictures++;
-        e->stats.d2h_bytes += g.out;
-    } while (0);
-    if (rc != SVT_B200_OK) {
-        cudaStreamSynchronize(s->st); // nothing of this picture may still read the planes
-        s->up_pending = false;
     }
-    plane_release(e, ents, n_ent);
-    release(e, s);
-    return rc;
+    DeviceGuard dg(e->device);
+    ENG_TRY(ensure_me(e, p));
+    const MeGeom &g = e->mg;
+    MeLease L(e);
+    MeSlot *s = L.s;
+    {
+        Lap lap(e->stats.ns_issue);
+        SvtB200MePlanes dsrc, drefs[SVT_B200_ME_LISTS][SVT_B200_ME_MAX_REFS] = {};
+        ENG_TRY(plane_acquire(e, L, p, src, filtered_downsample, &dsrc));
+        for (int l = 0; l < p->num_lists; l++)
+            for (int r = 0; r < p->num_refs[l]; r++) ENG_TRY(plane_acquire(e, L, p, &refs[l][r], filtered_downsample, &drefs[l][r]));
+        ENG_TRY(svt_b200_me_picture(p, &dsrc, drefs, &s->out, s->scratch, s->st));
+        ENG_TRY(copy_async(e, s->pin_mv, s->out.me_mv, g.out, cudaMemcpyDeviceToHost, s->st));
+    }
+    ENG_TRY(timed_sync(e, s->st));
+    L.done = true;
+    Lap lap(e->stats.ns_host_copy);
+    memcpy(me_mv, s->pin_mv, g.b_mv);
+    memcpy(me_cand, s->pin_cand, g.b_cand);
+    memcpy(total_cand, s->pin_tot, g.b_tot);
+    memcpy(rc_me_distortion, s->pin_rc, g.b_rc);
+    e->stats.me_pictures++;
+    return SVT_B200_OK;
 }
 
 int svt_b200_engine_dlf_frame(SvtB200Engine *e, const SvtB200DlfParams *p, const SvtB200Frame *frame, const SvtB200DlfMi *mi) {
@@ -610,44 +683,31 @@ int svt_b200_engine_dlf_frame(SvtB200Engine *e, const SvtB200DlfParams *p, const
         return SVT_B200_ERR_ARG;
     }
     DeviceGuard dg(e->device);
-    int rc = ensure_filt(e, frame->width, frame->height, frame->bit_depth, p->mi_rows, p->mi_cols);
-    if (rc != SVT_B200_OK) return rc;
-    const FiltGeom &g = e->fg;
+    ENG_TRY(ensure_filt(e, frame->width, frame->height, frame->bit_depth, p->mi_rows, p->mi_cols));
     const size_t b_mi = (size_t)p->mi_rows * p->mi_cols * sizeof(SvtB200DlfMi);
-    if (b_mi > g.mi) {
+    if (b_mi > e->fg.mi) {
         set_error("svt_b200_engine_dlf_frame: mode-info array larger than the sequence geometry");
         return SVT_B200_ERR_ARG;
     }
-    FiltSlot *s = acquire(e, e->filt);
-    do {
-        pack_frame(e, s->pin_a, frame);
-        {
-            Lap lap(e->stats.ns_host_copy);
-            par_memcpy(s->pin_b, mi, b_mi);
-        }
-        {
-            Lap lap(e->stats.ns_issue);
-            if (cudaMemcpyAsync(s->misc, s->pin_b, b_mi, cudaMemcpyHostToDevice, s->st) != cudaSuccess) {
-                set_error("engine: mode-info upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            if ((rc = copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st)) != SVT_B200_OK) break;
-            if ((rc = svt_b200_dlf_frame(p, &s->recon, (const SvtB200DlfMi *)s->misc, s->st)) != SVT_B200_OK) break;
-            if ((rc = copy_packed(e, &s->recon, s->pin_a, cudaMemcpyDeviceToHost, s->st)) != SVT_B200_OK) break;
-        }
-        if (timed_sync(e, s->st) != cudaSuccess) {
-            set_error("engine: deblocking failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = SVT_B200_ERR_CUDA;
-            break;
-        }
-        unpack_frame(e, frame, s->pin_a);
-        e->stats.dlf_frames++;
-        e->stats.h2d_bytes += b_mi;
-    } while (0);
-    if (rc != SVT_B200_OK) cudaStreamSynchronize(s->st);
-    release(e, s);
-    return rc;
+    FiltLease L(e);
+    FiltSlot *s = L.s;
+    pack_frame(e, s->pin_a, frame);
+    {
+        Lap lap(e->stats.ns_host_copy);
+        par_memcpy(s->pin_mi, mi, b_mi);
+    }
+    {
+        Lap lap(e->stats.ns_issue);
+        ENG_TRY(copy_async(e, s->mi, s->pin_mi, b_mi, cudaMemcpyHostToDevice, s->st));
+        ENG_TRY(copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st));
+        ENG_TRY(svt_b200_dlf_frame(p, &s->recon, s->mi, s->st));
+        ENG_TRY(copy_packed(e, &s->recon, s->pin_a, cudaMemcpyDeviceToHost, s->st));
+    }
+    ENG_TRY(timed_sync(e, s->st));
+    L.done = true;
+    unpack_frame(e, frame, s->pin_a);
+    e->stats.dlf_frames++;
+    return SVT_B200_OK;
 }
 
 int svt_b200_engine_dlf_pick_frame(SvtB200Engine *e, const SvtB200LpfPickParams *pp, const SvtB200Frame *recon,
@@ -658,66 +718,45 @@ int svt_b200_engine_dlf_pick_frame(SvtB200Engine *e, const SvtB200LpfPickParams 
         return SVT_B200_ERR_ARG;
     }
     DeviceGuard dg(e->device);
-    int rc = ensure_filt(e, recon->width, recon->height, recon->bit_depth, pp->dlf.mi_rows, pp->dlf.mi_cols);
-    if (rc != SVT_B200_OK) return rc;
-    const FiltGeom &g = e->fg;
+    ENG_TRY(ensure_filt(e, recon->width, recon->height, recon->bit_depth, pp->dlf.mi_rows, pp->dlf.mi_cols));
     const size_t b_mi = (size_t)pp->dlf.mi_rows * pp->dlf.mi_cols * sizeof(SvtB200DlfMi);
-    if (b_mi > g.mi) {
+    if (b_mi > e->fg.mi) {
         set_error("svt_b200_engine_dlf_pick_frame: mode-info array larger than the sequence geometry");
         return SVT_B200_ERR_ARG;
     }
-    FiltSlot *s = acquire(e, e->filt);
-    do {
-        uint8_t *d_scratch = s->misc + g.mi; // 768 B level table + the SSE accumulator of the search, then the final table
-        pack_frame(e, s->pin_a, recon);
-        {
-            Lap lap(e->stats.ns_issue);
-            if ((rc = copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st)) != SVT_B200_OK) break;
-        }
-        // pin_b holds the mode-info array first, then (after its upload completed) the packed source picture
-        {
-            Lap lap(e->stats.ns_host_copy);
-            par_memcpy(s->pin_b, mi, b_mi);
-        }
-        if (cudaMemcpyAsync(s->misc, s->pin_b, b_mi, cudaMemcpyHostToDevice, s->st) != cudaSuccess || timed_sync(e, s->st) != cudaSuccess) {
-            set_error("engine: mode-info upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = SVT_B200_ERR_CUDA;
-            break;
-        }
-        pack_frame(e, s->pin_b, source);
-        if ((rc = copy_packed(e, &s->source, s->pin_b, cudaMemcpyHostToDevice, s->st)) != SVT_B200_OK) break;
-        // every trial: one plane pass + SSE + plane restore on the device, one 8-byte read-back (the bisection is host logic)
-        if ((rc = svt_b200_pick_filter_level(pp, &s->recon, &s->source, &s->out, (const SvtB200DlfMi *)s->misc, d_scratch, levels_out,
-                                             s->st)) != SVT_B200_OK)
-            break;
-        SvtB200DlfParams dp = pp->dlf;
-        dp.sharpness = 0; // svt_av1_pick_filter_level sets lf->sharpness_level = 0 (EbDeblockingFilter.c:1202)
-        dp.filter_level[0] = levels_out[0], dp.filter_level[1] = levels_out[1];
-        dp.filter_level_u = levels_out[2], dp.filter_level_v = levels_out[3];
-        dp.plane_start = 0, dp.plane_end = 3;
-        uint8_t(*lut)[2][128] = reinterpret_cast<uint8_t(*)[2][128]>(s->pin_small);
-        svt_b200_lf_level_lut(&pp->init, levels_out, lut);
-        {
-            Lap lap(e->stats.ns_issue);
-            if (cudaMemcpyAsync(d_scratch + 1024, s->pin_small, 768, cudaMemcpyHostToDevice, s->st) != cudaSuccess) {
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            if ((rc = svt_b200_dlf_frame_lut(&dp, &s->recon, (const SvtB200DlfMi *)s->misc, d_scratch + 1024, s->st)) != SVT_B200_OK) break;
-            if ((rc = copy_packed(e, &s->recon, s->pin_a, cudaMemcpyDeviceToHost, s->st)) != SVT_B200_OK) break;
-        }
-        if (timed_sync(e, s->st) != cudaSuccess) {
-            set_error("engine: deblocking (picked levels) failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = SVT_B200_ERR_CUDA;
-            break;
-        }
-        unpack_frame(e, recon, s->pin_a);
-        e->stats.dlf_frames++;
-        e->stats.h2d_bytes += b_mi;
-    } while (0);
-    if (rc != SVT_B200_OK) cudaStreamSynchronize(s->st);
-    release(e, s);
-    return rc;
+    FiltLease L(e);
+    FiltSlot *s = L.s;
+    pack_frame(e, s->pin_a, recon);
+    {
+        Lap lap(e->stats.ns_issue);
+        ENG_TRY(copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st));
+    }
+    {
+        Lap lap(e->stats.ns_host_copy);
+        par_memcpy(s->pin_mi, mi, b_mi);
+    }
+    ENG_TRY(copy_async(e, s->mi, s->pin_mi, b_mi, cudaMemcpyHostToDevice, s->st));
+    pack_frame(e, s->pin_b, source);
+    ENG_TRY(copy_packed(e, &s->source, s->pin_b, cudaMemcpyHostToDevice, s->st));
+    // every trial: one plane pass + SSE + plane restore on the device, one 8-byte read-back (the bisection is host logic)
+    ENG_TRY(svt_b200_pick_filter_level(pp, &s->recon, &s->source, &s->out, s->mi, s->pick, levels_out, s->st));
+    SvtB200DlfParams dp = pp->dlf;
+    dp.sharpness = 0; // svt_av1_pick_filter_level sets lf->sharpness_level = 0 (EbDeblockingFilter.c:1202)
+    dp.filter_level[0] = levels_out[0], dp.filter_level[1] = levels_out[1];
+    dp.filter_level_u = levels_out[2], dp.filter_level_v = levels_out[3];
+    dp.plane_start = 0, dp.plane_end = 3;
+    svt_b200_lf_level_lut(&pp->init, levels_out, reinterpret_cast<uint8_t(*)[2][128]>(s->pin_small));
+    {
+        Lap lap(e->stats.ns_issue);
+        ENG_TRY(copy_async(e, s->lut, s->pin_small, kLutBytes, cudaMemcpyHostToDevice, s->st));
+        ENG_TRY(svt_b200_dlf_frame_lut(&dp, &s->recon, s->mi, s->lut, s->st));
+        ENG_TRY(copy_packed(e, &s->recon, s->pin_a, cudaMemcpyDeviceToHost, s->st));
+    }
+    ENG_TRY(timed_sync(e, s->st));
+    L.done = true;
+    unpack_frame(e, recon, s->pin_a);
+    e->stats.dlf_frames++;
+    return SVT_B200_OK;
 }
 
 int svt_b200_engine_lr_frame(SvtB200Engine *e, const SvtB200LrFrameParams *p, const int32_t n_units[3], const SvtB200Frame *frame,
@@ -727,123 +766,88 @@ int svt_b200_engine_lr_frame(SvtB200Engine *e, const SvtB200LrFrameParams *p, co
         return SVT_B200_ERR_ARG;
     }
     DeviceGuard dg(e->device);
-    int rc = ensure_filt(e, frame->width, frame->height, frame->bit_depth, (frame->height + 3) / 4, (frame->width + 3) / 4);
-    if (rc != SVT_B200_OK) return rc;
+    ENG_TRY(ensure_filt(e, frame->width, frame->height, frame->bit_depth, (frame->height + 3) / 4, (frame->width + 3) / 4));
     const FiltGeom &g = e->fg;
-    const int bps = frame->bit_depth > 8 ? 2 : 1;
+    const Packed pk(frame);
     size_t b_units = 0;
     for (int i = 0; i < 3; i++) b_units += al256((size_t)std::max(n_units[i], 0) * sizeof(SvtB200LrUnit));
     // staging of the boundary lines: 4 rows per stripe boundary and plane
     size_t b_lines = 0;
-    int nb[3], pw[3], ph[3], SH[3], off[3];
+    int nb[3], SH[3], off[3];
+    unsigned restored = 0; // planes with restoration; the others stay as they are on the host, as in the reference
     for (int i = 0; i < 3; i++) {
         const int ss = i ? 1 : 0;
-        pw[i] = i ? (frame->width + 1) >> 1 : frame->width;
-        ph[i] = i ? (frame->height + 1) >> 1 : frame->height;
         SH[i] = 64 >> ss, off[i] = 8 >> ss;
-        const int n_stripes = (ph[i] + off[i] + SH[i] - 1) / SH[i];
+        const int n_stripes = (pk.h[i] + off[i] + SH[i] - 1) / SH[i];
         nb[i] = p->plane[i].frame_restoration_type ? n_stripes - 1 : 0;
-        b_lines += al256((size_t)nb[i] * 4 * pw[i] * bps);
+        if (p->plane[i].frame_restoration_type) restored |= 1u << i;
+        b_lines += al256((size_t)nb[i] * 4 * pk.row[i]);
     }
     if (b_units + 256 > g.misc || b_lines > g.packed) {
         set_error("svt_b200_engine_lr_frame: unit / boundary-line arrays larger than the sequence geometry");
         return SVT_B200_ERR_ARG;
     }
-    FiltSlot *s = acquire(e, e->filt);
-    do {
-        pack_frame(e, s->pin_a, frame);
-        // units -> pin_small (host) -> misc (device)
-        SvtB200LrFrameParams dp = *p;
-        {
-            size_t o = 0;
-            if (b_units > g.small) {
-                set_error("svt_b200_engine_lr_frame: too many restoration units");
-                rc = SVT_B200_ERR_ARG;
-                break;
+    if (b_units > g.small) {
+        set_error("svt_b200_engine_lr_frame: too many restoration units");
+        return SVT_B200_ERR_ARG;
+    }
+    FiltLease L(e);
+    FiltSlot *s = L.s;
+    pack_frame(e, s->pin_a, frame);
+    // units -> pin_small (host) -> the slot's device region from s->mi on, each plane's array 256-byte aligned
+    SvtB200LrFrameParams dp = *p;
+    size_t o = 0;
+    for (int i = 0; i < 3; i++) {
+        const size_t n = (size_t)std::max(n_units[i], 0) * sizeof(SvtB200LrUnit);
+        if (n) memcpy(s->pin_small + o, p->plane[i].units, n);
+        dp.plane[i].units = (const SvtB200LrUnit *)((uint8_t *)s->mi + o);
+        o += al256(n);
+    }
+    // boundary lines: [boundary][row -2, -1, 0, +1 around the stripe edge][width], packed per plane in pin_b
+    {
+        Lap lap(e->stats.ns_host_copy);
+        o = 0;
+        for (int i = 0; i < 3; i++) {
+            const size_t rb = pk.row[i], ls = (size_t)lines[i].stride * pk.bps;
+            for (int b = 0; b < nb[i]; b++) {
+                uint8_t *d = s->pin_b + o + (size_t)b * 4 * rb;
+                const uint8_t *ab = (const uint8_t *)lines[i].above + (size_t)(2 * (b + 1)) * ls; // stripe b+1: rows y0-2, y0-1
+                const uint8_t *be = (const uint8_t *)lines[i].below + (size_t)(2 * b) * ls;       // stripe b: rows y1, y1+1
+                memcpy(d, ab, rb);
+                memcpy(d + rb, ab + ls, rb);
+                memcpy(d + 2 * rb, be, rb);
+                memcpy(d + 3 * rb, be + ls, rb);
             }
-            for (int i = 0; i < 3; i++) {
-                const size_t n = (size_t)std::max(n_units[i], 0) * sizeof(SvtB200LrUnit);
-                if (n) memcpy(s->pin_small + o, p->plane[i].units, n);
-                dp.plane[i].units = (const SvtB200LrUnit *)(s->misc + o);
-                o += al256(n);
-            }
+            o += al256((size_t)nb[i] * 4 * rb);
         }
-        // boundary lines: [boundary][row -2, -1, 0, +1 around the stripe edge][width], packed per plane in pin_b
-        {
-            Lap lap(e->stats.ns_host_copy);
-            size_t o = 0;
-            for (int i = 0; i < 3; i++) {
-                const size_t rb = (size_t)pw[i] * bps, ls = (size_t)lines[i].stride * bps;
-                for (int b = 0; b < nb[i]; b++) {
-                    uint8_t *d = s->pin_b + o + (size_t)b * 4 * rb;
-                    const uint8_t *ab = (const uint8_t *)lines[i].above + (size_t)(2 * (b + 1)) * ls; // stripe b+1: rows y0-2, y0-1
-                    const uint8_t *be = (const uint8_t *)lines[i].below + (size_t)(2 * b) * ls;       // stripe b: rows y1, y1+1
-                    memcpy(d, ab, rb);
-                    memcpy(d + rb, ab + ls, rb);
-                    memcpy(d + 2 * rb, be, rb);
-                    memcpy(d + 3 * rb, be + ls, rb);
-                }
-                o += al256((size_t)nb[i] * 4 * rb);
+    }
+    {
+        Lap lap(e->stats.ns_issue);
+        if (b_units) ENG_TRY(copy_async(e, s->mi, s->pin_small, b_units, cudaMemcpyHostToDevice, s->st));
+        ENG_TRY(copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st));
+        // scatter the boundary rows into a device picture that is only read at those rows (the deblocked context)
+        const Packed ctx(&s->source);
+        o = 0;
+        for (int i = 0; i < 3; i++) {
+            if (!nb[i]) continue;
+            const size_t rb = pk.row[i];
+            for (int k = 0; k < 4; k++) { // row B - 2 + k of every boundary B = (b + 1) * SH - off
+                int rows = nb[i];
+                if (nb[i] * SH[i] - off[i] - 2 + k >= pk.h[i]) rows--; // the last boundary's row lies below the plane
+                if (rows <= 0) continue;
+                ENG_TRY(copy_2d_async(e, ctx.plane[i] + (size_t)(SH[i] - off[i] - 2 + k) * ctx.pitch[i], ctx.pitch[i] * SH[i],
+                                      s->pin_b + o + (size_t)k * rb, 4 * rb, rb, rows, cudaMemcpyHostToDevice, s->st));
             }
+            o += al256((size_t)nb[i] * 4 * rb);
         }
-        {
-            Lap lap(e->stats.ns_issue);
-            if (b_units && cudaMemcpyAsync(s->misc, s->pin_small, b_units, cudaMemcpyHostToDevice, s->st) != cudaSuccess) {
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            if ((rc = copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st)) != SVT_B200_OK) break;
-            // scatter the boundary rows into a device picture that is only read at those rows (the deblocked context)
-            size_t o = 0;
-            bool ok = true;
-            for (int i = 0; i < 3 && ok; i++) {
-                if (!nb[i]) continue;
-                const size_t rb = (size_t)pw[i] * bps;
-                uint8_t *plane = (uint8_t *)(i == 0 ? s->source.y : i == 1 ? s->source.cb : s->source.cr);
-                const size_t dpitch = (size_t)(i ? s->source.stride_c : s->source.stride_y) * bps;
-                for (int k = 0; k < 4 && ok; k++) { // row B - 2 + k of every boundary B = (b + 1) * SH - off
-                    int rows = nb[i];
-                    if ((nb[i]) * SH[i] - off[i] - 2 + k >= ph[i]) rows--; // the last boundary's row lies below the plane
-                    if (rows <= 0) continue;
-                    ok = cudaMemcpy2DAsync(plane + (size_t)(SH[i] - off[i] - 2 + k) * dpitch, dpitch * SH[i], s->pin_b + o + (size_t)k * rb,
-                                           4 * rb, rb, rows, cudaMemcpyHostToDevice, s->st) == cudaSuccess;
-                }
-                o += al256((size_t)nb[i] * 4 * rb);
-            }
-            if (!ok) {
-                set_error("engine: boundary-line upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            if ((rc = svt_b200_lr_frame(&dp, &s->recon, &s->source, &s->out, s->st)) != SVT_B200_OK) break;
-            if ((rc = copy_packed(e, &s->out, s->pin_a, cudaMemcpyDeviceToHost, s->st)) != SVT_B200_OK) break;
-        }
-        if (timed_sync(e, s->st) != cudaSuccess) {
-            set_error("engine: loop restoration failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = SVT_B200_ERR_CUDA;
-            break;
-        }
-        // planes without restoration stay as they are on the host (the reference copies back only filtered planes)
-        SvtB200Frame fr = *frame;
-        {
-            Lap lap(e->stats.ns_host_copy);
-            const int cw = pw[1], ch = ph[1];
-            const size_t rw = (size_t)frame->width * bps, rcb = (size_t)cw * bps;
-            const uint8_t *py = s->pin_a, *pcb = py + rw * frame->height, *pcr = pcb + rcb * ch;
-            if (p->plane[0].frame_restoration_type) {
-                const RowCopy c[3] = {{(uint8_t *)fr.y, py, (size_t)fr.stride_y * bps, rw, rw, fr.height}, {nullptr, nullptr, 0, 0, 0, 0}, {nullptr, nullptr, 0, 0, 0, 0}};
-                run_copies(e, c);
-            }
-            if (p->plane[1].frame_restoration_type)
-                for (int y = 0; y < ch; y++) memcpy((uint8_t *)fr.cb + (size_t)y * fr.stride_c * bps, pcb + y * rcb, rcb);
-            if (p->plane[2].frame_restoration_type)
-                for (int y = 0; y < ch; y++) memcpy((uint8_t *)fr.cr + (size_t)y * fr.stride_c * bps, pcr + y * rcb, rcb);
-        }
-        e->stats.lr_frames++;
-    } while (0);
-    if (rc != SVT_B200_OK) cudaStreamSynchronize(s->st);
-    release(e, s);
-    return rc;
+        ENG_TRY(svt_b200_lr_frame(&dp, &s->recon, &s->source, &s->out, s->st));
+        ENG_TRY(copy_packed(e, &s->out, s->pin_a, cudaMemcpyDeviceToHost, s->st));
+    }
+    ENG_TRY(timed_sync(e, s->st));
+    L.done = true;
+    unpack_frame(e, frame, s->pin_a, restored);
+    e->stats.lr_frames++;
+    return SVT_B200_OK;
 }
 
 // The CDEF stage of one picture, with the deblocking the DLF stage deferred (dlf != NULL) and the strength decision on
@@ -860,78 +864,52 @@ int svt_b200_engine_dlf_cdef_frame_dev(SvtB200Engine *e, const SvtB200DlfParams 
         return SVT_B200_ERR_ARG;
     }
     DeviceGuard dg(e->device);
-    int rc = ensure_filt(e, recon->width, recon->height, recon->bit_depth, sp->mi_rows, sp->mi_cols);
-    if (rc != SVT_B200_OK) return rc;
+    ENG_TRY(ensure_filt(e, recon->width, recon->height, recon->bit_depth, sp->mi_rows, sp->mi_cols));
     const FiltGeom &g = e->fg;
-    const int nvfb = (sp->mi_rows + 15) / 16, nhfb = (sp->mi_cols + 15) / 16, nfb = nvfb * nhfb;
+    const int nfb = ((sp->mi_rows + 15) / 16) * ((sp->mi_cols + 15) / 16);
     const size_t b_skip = (size_t)((sp->mi_rows + 1) / 2) * skip_stride;
     const size_t b_mi = dlf ? (size_t)dlf->mi_rows * dlf->mi_cols * sizeof(SvtB200DlfMi) : 0;
     if (al256(b_skip) > g.skip || (size_t)nfb > g.nfb || b_mi > g.mi) {
         set_error("svt_b200_engine_dlf_cdef_frame_dev: picture larger than the sequence geometry");
         return SVT_B200_ERR_ARG;
     }
-    FiltSlot *s = acquire(e, e->filt);
-    do {
-        uint8_t *d_small = s->misc + g.mi + 4096;
-        uint8_t *d_skip = d_small, *d_mse = d_small + g.skip, *d_idx = d_mse + g.mse, *d_dec = d_idx + g.idx;
-        uint8_t *d_scr = d_dec + al256(sizeof(SvtB200CdefDecision));
-        uint8_t *h_skip = s->pin_small, *h_idx = h_skip + g.skip + g.mse;
-        pack_frame(e, s->pin_a, recon);
-        {
-            Lap lap(e->stats.ns_host_copy);
-            if (dlf) par_memcpy(s->pin_mi, mi, b_mi);
-            memcpy(h_skip, skip8, b_skip);
+    FiltLease L(e);
+    FiltSlot *s = L.s;
+    pack_frame(e, s->pin_a, recon);
+    {
+        Lap lap(e->stats.ns_host_copy);
+        if (dlf) par_memcpy(s->pin_mi, mi, b_mi);
+        memcpy(s->pin_small, skip8, b_skip);
+    }
+    {
+        Lap lap(e->stats.ns_issue);
+        if (dlf) ENG_TRY(copy_async(e, s->mi, s->pin_mi, b_mi, cudaMemcpyHostToDevice, s->st));
+        ENG_TRY(copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st));
+        if (dlf) ENG_TRY(svt_b200_dlf_frame(dlf, &s->recon, s->mi, s->st));
+    }
+    pack_frame(e, s->pin_b, source); // the host packs the source while the device receives and deblocks the reconstruction
+    {
+        Lap lap(e->stats.ns_issue);
+        ENG_TRY(copy_async(e, s->skip, s->pin_small, b_skip, cudaMemcpyHostToDevice, s->st));
+        ENG_TRY(copy_packed(e, &s->source, s->pin_b, cudaMemcpyHostToDevice, s->st));
+        ENG_TRY(svt_b200_cdef_search(sp, &s->recon, &s->source, s->skip, skip_stride, s->mse, s->st));
+        ENG_TRY(svt_b200_cdef_decide(dp, s->mse, s->skip, skip_stride, s->dec, s->idx, s->decide, s->st));
+        if (apply) {
+            ENG_TRY(svt_b200_cdef_apply_dev(sp->mi_rows, sp->mi_cols, damping, s->dec, &s->recon, &s->out, s->skip, skip_stride, s->idx,
+                                            s->st));
+            ENG_TRY(copy_packed(e, &s->out, s->pin_a, cudaMemcpyDeviceToHost, s->st));
         }
-        {
-            Lap lap(e->stats.ns_issue);
-            if (dlf && cudaMemcpyAsync(s->misc, s->pin_mi, b_mi, cudaMemcpyHostToDevice, s->st) != cudaSuccess) {
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            if ((rc = copy_packed(e, &s->recon, s->pin_a, cudaMemcpyHostToDevice, s->st)) != SVT_B200_OK) break;
-            if (dlf && (rc = svt_b200_dlf_frame(dlf, &s->recon, (const SvtB200DlfMi *)s->misc, s->st)) != SVT_B200_OK) break;
-        }
-        pack_frame(e, s->pin_b, source); // the host packs the source while the device receives and deblocks the reconstruction
-        {
-            Lap lap(e->stats.ns_issue);
-            if (cudaMemcpyAsync(d_skip, h_skip, b_skip, cudaMemcpyHostToDevice, s->st) != cudaSuccess) {
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-            if ((rc = copy_packed(e, &s->source, s->pin_b, cudaMemcpyHostToDevice, s->st)) != SVT_B200_OK) break;
-            if ((rc = svt_b200_cdef_search(sp, &s->recon, &s->source, d_skip, skip_stride, (uint64_t *)d_mse, s->st)) != SVT_B200_OK)
-                break;
-            if ((rc = svt_b200_cdef_decide(dp, (const uint64_t *)d_mse, d_skip, skip_stride, (SvtB200CdefDecision *)d_dec, (int8_t *)d_idx,
-                                           d_scr, s->st)) != SVT_B200_OK)
-                break;
-            if (apply) {
-                if ((rc = svt_b200_cdef_apply_dev(sp->mi_rows, sp->mi_cols, damping, (const SvtB200CdefDecision *)d_dec, &s->recon, &s->out,
-                                                  d_skip, skip_stride, (const int8_t *)d_idx, s->st)) != SVT_B200_OK)
-                    break;
-                if ((rc = copy_packed(e, &s->out, s->pin_a, cudaMemcpyDeviceToHost, s->st)) != SVT_B200_OK) break;
-            }
-            // filter-block indices and the decision are adjacent on both sides: one copy
-            if (cudaMemcpyAsync(h_idx, d_idx, g.idx + sizeof(SvtB200CdefDecision), cudaMemcpyDeviceToHost, s->st) != cudaSuccess) {
-                rc = SVT_B200_ERR_CUDA;
-                break;
-            }
-        }
-        if (timed_sync(e, s->st) != cudaSuccess) {
-            set_error("engine: deblocking + CDEF failed: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = SVT_B200_ERR_CUDA;
-            break;
-        }
-        memcpy(fb_strength_idx, h_idx, (size_t)nfb);
-        memcpy(decision, h_idx + g.idx, sizeof(SvtB200CdefDecision));
-        if (apply) unpack_frame(e, recon, s->pin_a);
-        if (dlf) e->stats.dlf_frames++;
-        e->stats.cdef_frames++;
-        e->stats.h2d_bytes += b_skip + b_mi;
-        e->stats.d2h_bytes += g.idx + sizeof(SvtB200CdefDecision);
-    } while (0);
-    if (rc != SVT_B200_OK) cudaStreamSynchronize(s->st);
-    release(e, s);
-    return rc;
+        // filter-block indices and the decision are adjacent on both sides: one copy
+        ENG_TRY(copy_async(e, s->pin_idx, s->idx, g.idx + sizeof(SvtB200CdefDecision), cudaMemcpyDeviceToHost, s->st));
+    }
+    ENG_TRY(timed_sync(e, s->st));
+    L.done = true;
+    memcpy(fb_strength_idx, s->pin_idx, (size_t)nfb);
+    memcpy(decision, s->pin_dec, sizeof(SvtB200CdefDecision));
+    if (apply) unpack_frame(e, recon, s->pin_a);
+    if (dlf) e->stats.dlf_frames++;
+    e->stats.cdef_frames++;
+    return SVT_B200_OK;
 }
 
 } // extern "C"

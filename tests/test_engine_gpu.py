@@ -12,15 +12,6 @@ import svtb200 as sb
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module")
-def engine():
-    lib = sb.load()
-    e = C.c_void_p()
-    sb.check(lib.svt_b200_engine_create(0, C.byref(e)), lib)
-    yield lib, e
-    lib.svt_b200_engine_destroy(e)
-
-
 def _host_pic(key, tag, planes, with_decimations=True):
     h = sb.HostMePicture()
     h.key, h.tag, h.full = key, tag, planes[0].ctypes.data
@@ -114,10 +105,10 @@ def test_engine_me_device_side_downsample_matches_uploaded_planes():
 # 1920x1080 10-bit: the packed picture (6.2 MB) is staged by the split host copy
 @pytest.mark.parametrize("case", [(320, 192, 8, 6, (12, 30, 0, 22), 2), (192, 136, 10, 2, (33, 17, 40, 25), 3),
                                   (1920, 1080, 10, 7, (36, 28, 20, 14), 1)])
-def test_engine_dlf_frame(engine, case):
+def test_engine_dlf_frame(case):
     from test_dlf_gpu import flat_mi
     from test_oracle_dlf import dlf_case, dlf_params
-    lib, _ = engine
+    lib = sb.load()
     e = C.c_void_p()
     sb.check(lib.svt_b200_engine_create(0, C.byref(e)), lib)  # one geometry per engine
     try:

@@ -410,8 +410,8 @@ def _filter_small_bytes(w, h):
 
 
 def test_lr_frame_error_after_taking_a_slot_releases_it(lib, filter_program_8bit):
-    """Nine loop-restoration calls with more unit bytes than the slot's staging fail after taking a slot; a valid call
-    still completes afterwards, so each failing call handed its slot back.  In a thread: a lost slot hangs the call."""
+    """Nine loop-restoration calls with more unit bytes than a slot's staging are refused before they take a slot; a
+    valid call still completes afterwards, so no refused call kept a slot.  In a thread: a lost slot hangs the call."""
     lr = next(c for c in filter_program_8bit if c.kind == "lr")
     small, mi = _filter_small_bytes(lr.cdef.w, lr.cdef.h)
     n = (small + mi // 2) // C.sizeof(sb.LrUnit)  # more than the staging holds, less than the device side accepts
@@ -448,3 +448,116 @@ def test_lr_frame_error_after_taking_a_slot_releases_it(lib, filter_program_8bit
     finally:
         if not t.is_alive():
             eng.close()
+
+
+def test_me_call_with_a_missing_reference_is_refused_before_any_upload(lib, me_program):
+    """Nine ME calls whose second list0 reference has no planes, and one that names more list0 references than
+    SvtB200MeParams holds, are refused before they take a slot or upload a picture; a valid call still completes
+    afterwards.  In a thread: a lost slot hangs the call."""
+    prog = me_program
+    call = next(c for c in prog.calls if len(c[1]) == 2 and len(c[2]) == 1)
+    i, l0, l1, params = call[:4]
+    hs, hr = prog.host(i), (sb.HostMePicture * 8)()
+    hr[0], hr[4] = prog.host(l0[0]), prog.host(l1[0])  # hr[1]: list0 reference 1 without planes
+    too_many = type(params).from_buffer_copy(params)
+    too_many.num_refs[0] = 5
+    got = cm.MeBuffers(prog.n_sb)
+    eng = Engine(lib)
+    out = {}
+
+    def me(p):
+        rc = lib.svt_b200_engine_me_picture(eng.e, C.byref(p), C.byref(hs), hr, 1, cm.ptr(got.me_mv), cm.ptr(got.me_cand),
+                                            cm.ptr(got.total_cand), cm.ptr(got.rc))
+        return rc, lib.svt_b200_last_error().decode()
+
+    def body():
+        try:
+            out["refused"] = [me(params) for _ in range(9)]
+            out["too_many"] = me(too_many)
+            out["uploads"] = eng.stats().me_plane_uploads
+            out["valid"] = MeCall(prog, call).run(lib, eng.e)
+        except Exception as ex:
+            out["exc"] = ex
+
+    try:
+        t = threading.Thread(target=body, daemon=True)
+        t.start()
+        t.join(timeout=120)
+        assert not t.is_alive(), "a call never got a slot: a refused call kept its slot"
+        assert "exc" not in out, out.get("exc")
+        assert all(rc == SVT_B200_ERR_ARG and "has no planes" in m for rc, m in out["refused"]), out["refused"]
+        assert out["too_many"][0] == SVT_B200_ERR_ARG and "more reference lists or references" in out["too_many"][1], out["too_many"]
+        assert out["uploads"] == 0
+        assert out["valid"] is None, out["valid"]
+        assert eng.stats().me_pictures == 1
+    finally:
+        if not t.is_alive():
+            eng.close()
+
+
+def _al256(v):
+    return (v + 255) & ~255
+
+
+def _packed_bytes(frame):
+    return sum(frame.plane(i).nbytes for i in range(3))
+
+
+def _filter_call_bytes(c):
+    """(H2D, D2H) bytes of one filter call: what the call must move between host staging and the device."""
+    mi = C.sizeof(sb.DlfMi)
+    if c.kind == "dlf":
+        pk = _packed_bytes(c.frame)
+        return pk + c.p.mi_rows * c.p.mi_cols * mi, pk
+    if c.kind == "pick":  # recon and source up, the mode info, the 768-byte level table of the picked levels
+        pk = _packed_bytes(c.rec)
+        return 2 * pk + c.p.dlf.mi_rows * c.p.dlf.mi_cols * mi + 3 * 2 * 128, pk
+    if c.kind == "cdef":  # recon and source up, the mode info when it deblocks, the skip map; down the index buffer + decision
+        ch = c.chain
+        pk = _packed_bytes(ch.rec)
+        up = 2 * pk + (ch.dp.mi_rows * ch.dp.mi_cols * mi if c.with_dlf else 0) + ((ch.sp.mi_rows + 1) // 2) * ch.skip.shape[1]
+        return up, (pk if c.apply else 0) + _al256(ch.nfb) + C.sizeof(sb.CdefDecision)
+    # lr: the units of every plane (each array 256-byte aligned, one copy), the picture, and in every restored plane the
+    # rows -2 .. +1 around each stripe boundary that lie inside the plane
+    pk = _packed_bytes(c.cdef)
+    up = sum(_al256(len(u) * C.sizeof(sb.LrUnit)) for u in c.units) + pk
+    for i in range(3):
+        if c.ftypes[i]:
+            plane = c.cdef.plane(i)
+            ph, row = plane.shape[0], plane.shape[1] * plane.itemsize
+            sh, off = 64 >> (i > 0), 8 >> (i > 0)
+            n_boundaries = (ph + off + sh - 1) // sh - 1
+            up += row * sum((b + 1) * sh - off - 2 + k < ph for b in range(n_boundaries) for k in range(4))
+    return up, pk
+
+
+def test_byte_counters_count_every_copy_once(lib, filter_program, me_program):
+    """h2d_bytes / d2h_bytes grow by exactly the bytes each call moves: every filter case of the geometry, then one ME
+    call whose four pictures are all uploaded with their decimations."""
+    eng = Engine(lib)
+    try:
+        fails = []
+        for c in filter_program:
+            before = eng.stats()
+            msg = c.run(lib, eng.e)
+            assert msg is None, f"{c.kind} [{c.name}]: {msg}"
+            after = eng.stats()
+            got = (after.h2d_bytes - before.h2d_bytes, after.d2h_bytes - before.d2h_bytes)
+            if got != _filter_call_bytes(c):
+                fails.append(f"{c.kind} [{c.name}]: (h2d, d2h) {got} != {_filter_call_bytes(c)}")
+        assert not fails, "\n".join(fails)
+        prog = me_program
+        call = next(c for c in prog.calls if len(set([c[0]] + c[1] + c[2])) == 4)
+        geos = prog.geos
+        nb = [g.stride * (g.height + 2 * g.origin_y) for g in geos]
+        before = eng.stats()
+        msg = MeCall(prog, call).run(lib, eng.e)
+        assert msg is None, msg
+        after = eng.stats()
+        assert after.me_plane_uploads - before.me_plane_uploads == 4
+        n_sb = prog.n_sb
+        want = (4 * (_al256(nb[0]) + _al256(nb[1]) + nb[2]),
+                _al256(n_sb * 85 * 7 * 4) + _al256(n_sb * 85 * 23) + _al256(n_sb * 85) + _al256(n_sb * 4))
+        assert (after.h2d_bytes - before.h2d_bytes, after.d2h_bytes - before.d2h_bytes) == want
+    finally:
+        eng.close()
