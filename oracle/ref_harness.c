@@ -50,24 +50,23 @@ static void plane_desc(EbPictureBufferDesc *d, const SvtB200Plane *g, const uint
     d->bit_depth = EB_8BIT;
 }
 
-/* Derive the preset's ME/HME parameters with the reference's own signal_derivation_me_kernel_oq
- * (EbMotionEstimationProcess.c:344) and run motion_estimate_sb (EbMotionEstimation.c:2912) over every SB
- * of one picture, with the per-SB set-up of motion_estimation_kernel (EbMotionEstimationProcess.c:831-940).
- * planes: src, then refs[list*4+idx]. */
-REFH_API int refh_me_picture(int width, int height, int enc_mode, int n_l0, int n_l1,
-                             const int32_t *ref_dist /*[8]*/, int temporal_layer, int is_ref,
-                             const SvtB200Plane *gfull, const SvtB200Plane *gquarter,
-                             const SvtB200Plane *gsixteenth, const SvtB200MePlanes *src,
-                             const SvtB200MePlanes *refs /*[8]*/, SvtB200MeParams *params_out,
-                             uint32_t *best_sad, uint32_t *best_mv, SvtB200HmeResult *hme, int16_t *me_mv,
-                             uint8_t *me_cand, uint8_t *total_cand, uint32_t *rc_me_distortion) {
-    refh_init();
-    SequenceControlSet *scs = calloc(1, sizeof(*scs));
-    PictureParentControlSet *pcs = calloc(1, sizeof(*pcs));
+/* Picture-level state of one ME call: what motion_estimation_kernel's caller sets up before
+ * signal_derivation_me_kernel_oq (EbMotionEstimationProcess.c:344) derives the preset's ME/HME parameters. */
+typedef struct {
+    SequenceControlSet *scs;
+    PictureParentControlSet *pcs;
     EbObjectWrapper scs_wrap;
-    memset(&scs_wrap, 0, sizeof(scs_wrap));
-    scs_wrap.object_ptr = scs;
-    pcs->scs_wrapper_ptr = &scs_wrap;
+    MotionEstimationContext_t mectx;
+    MeContext *me;
+} MeSetup;
+
+static MeSetup *me_setup_new(int width, int height, int enc_mode, int n_l0, int n_l1, int temporal_layer, int is_ref) {
+    refh_init();
+    MeSetup *s = calloc(1, sizeof(*s));
+    SequenceControlSet *scs = s->scs = calloc(1, sizeof(*scs));
+    PictureParentControlSet *pcs = s->pcs = calloc(1, sizeof(*pcs));
+    s->scs_wrap.object_ptr = scs;
+    pcs->scs_wrapper_ptr = &s->scs_wrap;
 
     /* sequence-level fields read by ME (EbEncHandle.c set_param_based_on_input / copy_api_from_app) */
     scs->static_config.use_default_me_hme = EB_TRUE;
@@ -102,6 +101,109 @@ REFH_API int refh_me_picture(int width, int height, int enc_mode, int n_l0, int 
     pcs->ref_list1_count_try = (uint8_t)n_l1;
     pcs->picture_number = 100;
 
+    s->me = calloc(1, sizeof(*s->me));
+    me_context_ctor(s->me);
+    s->mectx.me_context_ptr = s->me;
+    signal_derivation_me_kernel_oq(scs, pcs, &s->mectx);
+    return s;
+}
+
+static void me_setup_free(MeSetup *s) {
+    s->me->dctor(s->me);
+    free(s->me);
+    free(s->pcs);
+    free(s->scs);
+    free(s);
+}
+
+/* The derived parameters in the C-ABI's plain struct; -3 when the preset uses an HME decimation the ABI
+ * does not describe (ONE_DECIMATION_HME: MR / MRS at <= 720p). */
+static int me_export_params(const MeSetup *s, int n_l0, int n_l1, const int32_t *ref_dist /*[8]*/, int temporal_layer,
+                            int is_ref, const SvtB200Plane *gfull, const SvtB200Plane *gquarter,
+                            const SvtB200Plane *gsixteenth, SvtB200MeParams *p) {
+    const MeContext *me = s->me;
+    memset(p, 0, sizeof(*p));
+    p->full = *gfull;
+    p->quarter = *gquarter;
+    p->sixteenth = *gsixteenth;
+    p->num_lists = n_l1 > 0 ? 2 : 1;
+    p->num_refs[0] = n_l0;
+    p->num_refs[1] = n_l1;
+    for (int i = 0; i < 8; i++) p->ref_dist[i / 4][i % 4] = ref_dist[i];
+    p->temporal_layer_index = temporal_layer;
+    p->is_used_as_reference_flag = is_ref;
+    p->enable_hme_flag = me->enable_hme_flag;
+    p->enable_hme_level0_flag = me->enable_hme_level0_flag;
+    p->enable_hme_level1_flag = me->enable_hme_level1_flag;
+    p->enable_hme_level2_flag = me->enable_hme_level2_flag;
+    p->hme_search_method = me->hme_search_method == SUB_SAD_SEARCH;
+    p->me_search_method = me->me_search_method == SUB_SAD_SEARCH;
+    p->number_hme_search_region_in_width = me->number_hme_search_region_in_width;
+    p->number_hme_search_region_in_height = me->number_hme_search_region_in_height;
+    p->hme_level0_total_search_area_width = me->hme_level0_total_search_area_width;
+    p->hme_level0_total_search_area_height = me->hme_level0_total_search_area_height;
+    p->hme_level0_max_total_search_area_width = me->hme_level0_max_total_search_area_width;
+    p->hme_level0_max_total_search_area_height = me->hme_level0_max_total_search_area_height;
+    for (int i = 0; i < 2; i++) {
+        p->hme_level0_search_area_in_width_array[i] = me->hme_level0_search_area_in_width_array[i];
+        p->hme_level0_search_area_in_height_array[i] = me->hme_level0_search_area_in_height_array[i];
+        p->hme_level0_max_search_area_in_width_array[i] = me->hme_level0_max_search_area_in_width_array[i];
+        p->hme_level0_max_search_area_in_height_array[i] = me->hme_level0_max_search_area_in_height_array[i];
+        p->hme_level1_search_area_in_width_array[i] = me->hme_level1_search_area_in_width_array[i];
+        p->hme_level1_search_area_in_height_array[i] = me->hme_level1_search_area_in_height_array[i];
+        p->hme_level2_search_area_in_width_array[i] = me->hme_level2_search_area_in_width_array[i];
+        p->hme_level2_search_area_in_height_array[i] = me->hme_level2_search_area_in_height_array[i];
+    }
+    p->search_area_width = me->search_area_width;
+    p->search_area_height = me->search_area_height;
+    p->max_me_search_width = me->max_me_search_width;
+    p->max_me_search_height = me->max_me_search_height;
+    p->enable_me_hme_ref_pruning = me->me_hme_prune_ctrls.enable_me_hme_ref_pruning;
+    p->prune_ref_if_hme_sad_dev_bigger_than_th = me->me_hme_prune_ctrls.prune_ref_if_hme_sad_dev_bigger_than_th;
+    p->prune_ref_if_me_sad_dev_bigger_than_th = me->me_hme_prune_ctrls.prune_ref_if_me_sad_dev_bigger_than_th;
+    p->enable_me_sr_adjustment = me->me_sr_adjustment_ctrls.enable_me_sr_adjustment;
+    p->reduce_me_sr_based_on_mv_length_th = me->me_sr_adjustment_ctrls.reduce_me_sr_based_on_mv_length_th;
+    p->stationary_hme_sad_abs_th = me->me_sr_adjustment_ctrls.stationary_hme_sad_abs_th;
+    p->stationary_me_sr_divisor = me->me_sr_adjustment_ctrls.stationary_me_sr_divisor;
+    p->reduce_me_sr_based_on_hme_sad_abs_th = me->me_sr_adjustment_ctrls.reduce_me_sr_based_on_hme_sad_abs_th;
+    p->me_sr_divisor_for_low_hme_sad = me->me_sr_adjustment_ctrls.me_sr_divisor_for_low_hme_sad;
+    p->max_number_of_pus_per_sb = s->pcs->max_number_of_pus_per_sb;
+    p->rc_dist_from_8x8 = s->scs->input_resolution <= INPUT_SIZE_480p_RANGE;
+    return me->hme_decimation != TWO_DECIMATION_HME ? -3 : 0;
+}
+
+/* The preset's ME/HME parameters only, exactly as refh_me_picture derives and exports them, without the search. */
+REFH_API int refh_me_params(int width, int height, int enc_mode, int n_l0, int n_l1, const int32_t *ref_dist /*[8]*/,
+                            int temporal_layer, int is_ref, const SvtB200Plane *gfull, const SvtB200Plane *gquarter,
+                            const SvtB200Plane *gsixteenth, SvtB200MeParams *params_out) {
+    MeSetup *s = me_setup_new(width, height, enc_mode, n_l0, n_l1, temporal_layer, is_ref);
+    const int rc = me_export_params(s, n_l0, n_l1, ref_dist, temporal_layer, is_ref, gfull, gquarter, gsixteenth, params_out);
+    me_setup_free(s);
+    return rc;
+}
+
+/* Derive the preset's ME/HME parameters (me_setup_new) and run motion_estimate_sb (EbMotionEstimation.c:2912)
+ * over every SB of one picture, with the per-SB set-up of motion_estimation_kernel
+ * (EbMotionEstimationProcess.c:831-940).  planes: src, then refs[list*4+idx]. */
+REFH_API int refh_me_picture(int width, int height, int enc_mode, int n_l0, int n_l1,
+                             const int32_t *ref_dist /*[8]*/, int temporal_layer, int is_ref,
+                             const SvtB200Plane *gfull, const SvtB200Plane *gquarter,
+                             const SvtB200Plane *gsixteenth, const SvtB200MePlanes *src,
+                             const SvtB200MePlanes *refs /*[8]*/, SvtB200MeParams *params_out,
+                             uint32_t *best_sad, uint32_t *best_mv, SvtB200HmeResult *hme, int16_t *me_mv,
+                             uint8_t *me_cand, uint8_t *total_cand, uint32_t *rc_me_distortion) {
+    MeSetup *s = me_setup_new(width, height, enc_mode, n_l0, n_l1, temporal_layer, is_ref);
+    PictureParentControlSet *pcs = s->pcs;
+    MeContext *me = s->me;
+    if (params_out) {
+        const int rc = me_export_params(s, n_l0, n_l1, ref_dist, temporal_layer, is_ref, gfull, gquarter, gsixteenth,
+                                        params_out);
+        if (rc) {
+            me_setup_free(s);
+            return rc;
+        }
+    }
+
     const int sbs_x = (width + 63) / 64, sbs_y = (height + 63) / 64, n_sb = sbs_x * sbs_y;
     pcs->sb_total_count = (uint16_t)n_sb;
     pcs->rc_me_distortion = calloc(n_sb, sizeof(uint32_t));
@@ -117,13 +219,6 @@ REFH_API int refh_me_picture(int width, int height, int enc_mode, int n_l0, int 
         memset(med.me_results[i]->total_me_candidate_index, 0, SQUARE_PU_COUNT);
     }
 
-    MotionEstimationContext_t mectx;
-    memset(&mectx, 0, sizeof(mectx));
-    MeContext *me = calloc(1, sizeof(*me));
-    me_context_ctor(me);
-    mectx.me_context_ptr = me;
-    signal_derivation_me_kernel_oq(scs, pcs, &mectx);
-
     EbPictureBufferDesc in_full, in_q, in_s, rf[8], rq[8], rs[8];
     plane_desc(&in_full, gfull, src->full);
     plane_desc(&in_q, gquarter, src->quarter);
@@ -132,59 +227,6 @@ REFH_API int refh_me_picture(int width, int height, int enc_mode, int n_l0, int 
         plane_desc(&rf[i], gfull, refs[i].full);
         plane_desc(&rq[i], gquarter, refs[i].quarter);
         plane_desc(&rs[i], gsixteenth, refs[i].sixteenth);
-    }
-
-    /* export the derived parameters in the C-ABI's plain struct */
-    if (params_out) {
-        SvtB200MeParams *p = params_out;
-        memset(p, 0, sizeof(*p));
-        p->full = *gfull;
-        p->quarter = *gquarter;
-        p->sixteenth = *gsixteenth;
-        p->num_lists = n_l1 > 0 ? 2 : 1;
-        p->num_refs[0] = n_l0;
-        p->num_refs[1] = n_l1;
-        for (int i = 0; i < 8; i++) p->ref_dist[i / 4][i % 4] = ref_dist[i];
-        p->temporal_layer_index = temporal_layer;
-        p->is_used_as_reference_flag = is_ref;
-        p->enable_hme_flag = me->enable_hme_flag;
-        p->enable_hme_level0_flag = me->enable_hme_level0_flag;
-        p->enable_hme_level1_flag = me->enable_hme_level1_flag;
-        p->enable_hme_level2_flag = me->enable_hme_level2_flag;
-        p->hme_search_method = me->hme_search_method == SUB_SAD_SEARCH;
-        p->me_search_method = me->me_search_method == SUB_SAD_SEARCH;
-        p->number_hme_search_region_in_width = me->number_hme_search_region_in_width;
-        p->number_hme_search_region_in_height = me->number_hme_search_region_in_height;
-        p->hme_level0_total_search_area_width = me->hme_level0_total_search_area_width;
-        p->hme_level0_total_search_area_height = me->hme_level0_total_search_area_height;
-        p->hme_level0_max_total_search_area_width = me->hme_level0_max_total_search_area_width;
-        p->hme_level0_max_total_search_area_height = me->hme_level0_max_total_search_area_height;
-        for (int i = 0; i < 2; i++) {
-            p->hme_level0_search_area_in_width_array[i] = me->hme_level0_search_area_in_width_array[i];
-            p->hme_level0_search_area_in_height_array[i] = me->hme_level0_search_area_in_height_array[i];
-            p->hme_level0_max_search_area_in_width_array[i] = me->hme_level0_max_search_area_in_width_array[i];
-            p->hme_level0_max_search_area_in_height_array[i] = me->hme_level0_max_search_area_in_height_array[i];
-            p->hme_level1_search_area_in_width_array[i] = me->hme_level1_search_area_in_width_array[i];
-            p->hme_level1_search_area_in_height_array[i] = me->hme_level1_search_area_in_height_array[i];
-            p->hme_level2_search_area_in_width_array[i] = me->hme_level2_search_area_in_width_array[i];
-            p->hme_level2_search_area_in_height_array[i] = me->hme_level2_search_area_in_height_array[i];
-        }
-        p->search_area_width = me->search_area_width;
-        p->search_area_height = me->search_area_height;
-        p->max_me_search_width = me->max_me_search_width;
-        p->max_me_search_height = me->max_me_search_height;
-        p->enable_me_hme_ref_pruning = me->me_hme_prune_ctrls.enable_me_hme_ref_pruning;
-        p->prune_ref_if_hme_sad_dev_bigger_than_th = me->me_hme_prune_ctrls.prune_ref_if_hme_sad_dev_bigger_than_th;
-        p->prune_ref_if_me_sad_dev_bigger_than_th = me->me_hme_prune_ctrls.prune_ref_if_me_sad_dev_bigger_than_th;
-        p->enable_me_sr_adjustment = me->me_sr_adjustment_ctrls.enable_me_sr_adjustment;
-        p->reduce_me_sr_based_on_mv_length_th = me->me_sr_adjustment_ctrls.reduce_me_sr_based_on_mv_length_th;
-        p->stationary_hme_sad_abs_th = me->me_sr_adjustment_ctrls.stationary_hme_sad_abs_th;
-        p->stationary_me_sr_divisor = me->me_sr_adjustment_ctrls.stationary_me_sr_divisor;
-        p->reduce_me_sr_based_on_hme_sad_abs_th = me->me_sr_adjustment_ctrls.reduce_me_sr_based_on_hme_sad_abs_th;
-        p->me_sr_divisor_for_low_hme_sad = me->me_sr_adjustment_ctrls.me_sr_divisor_for_low_hme_sad;
-        p->max_number_of_pus_per_sb = pcs->max_number_of_pus_per_sb;
-        p->rc_dist_from_8x8 = scs->input_resolution <= INPUT_SIZE_480p_RANGE;
-        if (me->hme_decimation != TWO_DECIMATION_HME) return -3;
     }
 
     for (int sy = 0; sy < sbs_y; sy++)
@@ -262,6 +304,13 @@ REFH_API int refh_me_picture(int width, int height, int enc_mode, int n_l0, int 
             }
             rc_me_distortion[sb] = pcs->rc_me_distortion[sb];
         }
+    for (int i = 0; i < n_sb; i++) {
+        med.me_results[i]->dctor(med.me_results[i]);
+        free(med.me_results[i]);
+    }
+    free(med.me_results);
+    free(pcs->rc_me_distortion);
+    me_setup_free(s);
     return 0;
 }
 

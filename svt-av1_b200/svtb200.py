@@ -218,11 +218,31 @@ class EngineStats(C.Structure):
                                           "ns_sync", "ns_host_copy")]
 
 
-def preset8_me_params(width, height, n_l0=1, n_l1=1, dist=((1, 2, 3, 4), (1, 2, 3, 4)), temporal_layer=1,
-                      is_ref=1):
-    """ME parameters of preset 8 (ENC_M8) at >=720p, 30 fps, as set_me_hme_params_oq /
-    signal_derivation_me_kernel_oq (EbMotionEstimationProcess.c:113-420) derive them.  tests check this table
-    against the reference's own derivation (oracle/_ref) when it is available."""
+# input-resolution classes (EbDefinitions.h ResolutionRange) and the luma sample counts that bound them
+RES_240P, RES_360P, RES_480P, RES_720P, RES_1080P, RES_4K, RES_8K = range(7)
+_RES_TH = (0x28500, 0x4CE00, 0xA1400, 0x16DA00, 0x535200, 0x140A000)
+PRESET_MRS, PRESET_MR = -2, -1
+
+
+def input_resolution(width, height):
+    """derive_input_resolution: the resolution class of a width x height picture."""
+    n = width * height
+    return next((i for i, th in enumerate(_RES_TH) if n < th), RES_8K)
+
+
+def me_params(preset, width, height, n_l0=1, n_l1=1, dist=((1, 2, 3, 4), (1, 2, 3, 4)), temporal_layer=1, is_ref=1,
+              input_resolution_class=None):
+    """ME parameters of `preset` (-2 = MRS .. 8) for non-screen content, default ME/HME, 30 fps, single pass, as
+    signal_derivation_me_kernel_oq derives them (EbMotionEstimationProcess.c:113-420: set_me_hme_params_oq,
+    set_me_hme_ref_prune_ctrls, set_me_sr_adjustment_ctrls).  `input_resolution_class` (RES_*) overrides the class
+    derived from width x height, so that a small picture can carry a larger class's table.  Raises ValueError where
+    the preset uses one-decimation HME (MR / MRS at <= 720p), which the library does not implement.  Tests check
+    this table against the reference's own derivation (oracle/_ref) when it is available."""
+    if not PRESET_MRS <= preset <= 8:
+        raise ValueError(f"preset {preset} out of range")
+    res = input_resolution(width, height) if input_resolution_class is None else input_resolution_class
+    if preset <= PRESET_MR and res <= RES_720P:
+        raise ValueError(f"preset {preset} at resolution class {res} uses one-decimation HME")
     p = MeParams()
     geo = me_geometry(width, height)
     p.full, p.quarter, p.sixteenth = geo
@@ -233,29 +253,56 @@ def preset8_me_params(width, height, n_l0=1, n_l1=1, dist=((1, 2, 3, 4), (1, 2, 
             p.ref_dist[l][r] = dist[l][r]
     p.temporal_layer_index, p.is_used_as_reference_flag = temporal_layer, is_ref
     p.enable_hme_flag = p.enable_hme_level0_flag = p.enable_hme_level1_flag = p.enable_hme_level2_flag = 1
-    p.hme_search_method = p.me_search_method = 1
+    p.hme_search_method = p.me_search_method = 0 if preset <= PRESET_MRS else 1  # full SAD at MRS, else sub-sampled
     p.number_hme_search_region_in_width = p.number_hme_search_region_in_height = 2
-    p.hme_level0_total_search_area_width = p.hme_level0_total_search_area_height = 32
-    p.hme_level0_max_total_search_area_width = p.hme_level0_max_total_search_area_height = 164
+    # full-pel search area (scaled by 3/2 below: 30 fps is a low frame rate) and its cap
+    if preset <= 2:
+        sa = 64
+        max_w = max_h = {0: 256, 1: 192, 2: 128}[max(preset, 0)]
+    elif preset <= 5:
+        sa, max_w, max_h = 16, 64, 64
+    else:
+        sa, max_w, max_h = 16, 64, 32
+    p.search_area_width = p.search_area_height = sa * 3 // 2
+    p.max_me_search_width, p.max_me_search_height = max_w, max_h
+    # HME level 0: total area over the 2x2 regions, each region gets half of it in each direction
+    if preset <= 1:
+        total, max_total = (120 if res <= RES_1080P else 240), 480
+    else:
+        total, max_total = 32, 164
+    p.hme_level0_total_search_area_width = p.hme_level0_total_search_area_height = total
+    p.hme_level0_max_total_search_area_width = p.hme_level0_max_total_search_area_height = max_total
+    l12_w, l12_h = (16, 16) if preset <= 4 else (8, 3)
     for i in range(2):
-        p.hme_level0_search_area_in_width_array[i] = p.hme_level0_search_area_in_height_array[i] = 16
-        p.hme_level0_max_search_area_in_width_array[i] = p.hme_level0_max_search_area_in_height_array[i] = 82
-        p.hme_level1_search_area_in_width_array[i] = p.hme_level2_search_area_in_width_array[i] = 8
-        p.hme_level1_search_area_in_height_array[i] = p.hme_level2_search_area_in_height_array[i] = 3
-    p.search_area_width = p.search_area_height = 24  # 16 * 3/2 (low frame rate)
-    p.max_me_search_width, p.max_me_search_height = 64, 32
-    p.enable_me_hme_ref_pruning = 1
-    p.prune_ref_if_hme_sad_dev_bigger_than_th = 30
-    p.prune_ref_if_me_sad_dev_bigger_than_th = 60
-    p.enable_me_sr_adjustment = 1
-    p.reduce_me_sr_based_on_mv_length_th = 4
-    p.stationary_hme_sad_abs_th = 12000
-    p.stationary_me_sr_divisor = 8
-    p.reduce_me_sr_based_on_hme_sad_abs_th = 6000
-    p.me_sr_divisor_for_low_hme_sad = 8
+        p.hme_level0_search_area_in_width_array[i] = p.hme_level0_search_area_in_height_array[i] = total // 2
+        p.hme_level0_max_search_area_in_width_array[i] = p.hme_level0_max_search_area_in_height_array[i] = max_total // 2
+        p.hme_level1_search_area_in_width_array[i] = p.hme_level2_search_area_in_width_array[i] = l12_w
+        p.hme_level1_search_area_in_height_array[i] = p.hme_level2_search_area_in_height_array[i] = l12_h
+    # HME / ME reference pruning: off at MR and MRS, level 2 at M0-M2, level 4 above
+    if preset <= PRESET_MR:
+        p.enable_me_hme_ref_pruning = 0
+        p.prune_ref_if_hme_sad_dev_bigger_than_th = p.prune_ref_if_me_sad_dev_bigger_than_th = 0xFFFF
+    else:
+        p.enable_me_hme_ref_pruning = 1
+        p.prune_ref_if_hme_sad_dev_bigger_than_th = 80 if preset <= 2 else 30
+        p.prune_ref_if_me_sad_dev_bigger_than_th = 60
+    # HME-based search-area adjustment: off at MRS (level 0 leaves the thresholds at zero), level 2 above
+    if preset > PRESET_MRS:
+        p.enable_me_sr_adjustment = 1
+        p.reduce_me_sr_based_on_mv_length_th = 4
+        p.stationary_hme_sad_abs_th = 12000
+        p.stationary_me_sr_divisor = 8
+        p.reduce_me_sr_based_on_hme_sad_abs_th = 6000
+        p.me_sr_divisor_for_low_hme_sad = 8
     p.max_number_of_pus_per_sb = 85
-    p.rc_dist_from_8x8 = 1 if width * height < 0xA1400 else 0
+    p.rc_dist_from_8x8 = 1 if res <= RES_480P else 0
     return p
+
+
+def preset8_me_params(width, height, n_l0=1, n_l1=1, dist=((1, 2, 3, 4), (1, 2, 3, 4)), temporal_layer=1,
+                      is_ref=1):
+    """ME parameters of preset 8 (ENC_M8), 30 fps: me_params(8, ...)."""
+    return me_params(8, width, height, n_l0, n_l1, dist, temporal_layer, is_ref)
 
 
 def me_geometry(width, height):
