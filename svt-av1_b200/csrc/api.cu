@@ -17,42 +17,85 @@ void set_error(const char *fmt, ...) {
     fprintf(stderr, "libsvtav1_b200: fatal CUDA error in %s: %s (no CPU fallback)\n", what, cudaGetErrorString(e));
     abort();
 }
-void ThreadCtx::drop() {
-    if (h) cudaFreeHost(h);
-    if (d) cudaFree(d);
-    if (stream) cudaStreamDestroy(stream);
-    h = d = nullptr;
-    stream = nullptr;
-    cap = 0;
-}
-void ThreadCtx::reserve(size_t bytes) {
-    int dev = 0;
-    SVTB_CUDA_FATAL(cudaGetDevice(&dev));
-    if (dev != device) { // this thread now serves another GPU: its stream and staging belong to the old one
-        if (device >= 0) {
-            cudaSetDevice(device);
-            drop();
-            cudaSetDevice(dev);
-        }
-        device = dev;
+namespace {
+// per-calling-thread stream + growable pinned/device buffers; only Staging reaches them
+struct ThreadCtx {
+    cudaStream_t stream = nullptr;
+    uint8_t *h = nullptr; // pinned
+    uint8_t *d = nullptr; // device
+    size_t cap = 0;
+    int device = -1; // the device stream / d belong to: rebuilt when the calling thread's current device changes
+    void free_buffers() {
+        if (h) cudaFreeHost(h);
+        if (d) cudaFree(d);
+        h = d = nullptr;
+        cap = 0;
     }
-    if (!stream) SVTB_CUDA_FATAL(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-    if (bytes <= cap) return;
-    size_t ncap = cap ? cap : (1u << 20);
-    while (ncap < bytes) ncap *= 2;
-    if (h) cudaFreeHost(h);
-    if (d) cudaFree(d);
-    SVTB_CUDA_FATAL(cudaMallocHost(&h, ncap));
-    SVTB_CUDA_FATAL(cudaMalloc(&d, ncap));
-    cap = ncap;
+    void drop() {
+        free_buffers();
+        if (stream) cudaStreamDestroy(stream);
+        stream = nullptr;
+    }
+    // on failure the buffers stay freed (cap 0), so the next call allocates again
+    cudaError_t reserve(size_t bytes) {
+        int dev = 0;
+        cudaError_t e = cudaGetDevice(&dev);
+        if (e != cudaSuccess) return e;
+        if (dev != device) { // this thread now serves another GPU: its stream and staging belong to the old one
+            if (device >= 0) {
+                cudaSetDevice(device);
+                drop();
+                cudaSetDevice(dev);
+            }
+            device = dev;
+        }
+        if (!stream && (e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking)) != cudaSuccess) return e;
+        if (bytes <= cap) return cudaSuccess;
+        size_t ncap = cap ? cap : (1u << 20);
+        while (ncap < bytes) ncap *= 2;
+        free_buffers();
+        void *nh = nullptr, *nd = nullptr;
+        if ((e = cudaMallocHost(&nh, ncap)) != cudaSuccess) return e;
+        if ((e = cudaMalloc(&nd, ncap)) != cudaSuccess) {
+            cudaFreeHost(nh);
+            return e;
+        }
+        h = (uint8_t *)nh, d = (uint8_t *)nd, cap = ncap;
+        return cudaSuccess;
+    }
+    ~ThreadCtx() {
+        // the CUDA context may already be gone at thread/process exit; ignore errors
+        drop();
+    }
+};
+thread_local ThreadCtx t_ctx;
+} // namespace
+
+Staging::Staging(std::initializer_list<size_t> region_bytes) {
+    if (region_bytes.size() > kMaxRegions) fatal("Staging: too many regions", cudaErrorInvalidValue);
+    size_t o = 0;
+    int n = 0;
+    for (size_t b : region_bytes) {
+        off_[n] = o;
+        bytes_[n++] = b;
+        o += (b + 255) & ~(size_t)255;
+    }
+    err_ = t_ctx.reserve(o);
+    if (err_ == cudaSuccess) h_ = t_ctx.h, d_ = t_ctx.d, st_ = t_ctx.stream;
 }
-ThreadCtx::~ThreadCtx() {
-    // the CUDA context may already be gone at thread/process exit; ignore errors
-    drop();
+void Staging::put_rows(int r, const void *src, ptrdiff_t stride, size_t es, size_t width, size_t rows) {
+    for (size_t y = 0; y < rows; y++) memcpy(h(r) + y * width * es, (const uint8_t *)src + (ptrdiff_t)y * stride * (ptrdiff_t)es, width * es);
 }
-ThreadCtx &tls() {
-    static thread_local ThreadCtx ctx;
-    return ctx;
+void Staging::get_rows(int r, void *dst, ptrdiff_t stride, size_t es, size_t width, size_t rows) const {
+    for (size_t y = 0; y < rows; y++) memcpy((uint8_t *)dst + (ptrdiff_t)y * stride * (ptrdiff_t)es, h(r) + y * width * es, width * es);
+}
+cudaError_t Staging::upload(int first, int last, size_t last_bytes) {
+    const size_t n = last_bytes < bytes_[last] ? span(first, last) - bytes_[last] + last_bytes : span(first, last);
+    return cudaMemcpyAsync(d(first), h(first), n, cudaMemcpyHostToDevice, st_);
+}
+cudaError_t Staging::download(int first, int last) {
+    const cudaError_t e = cudaMemcpyAsync(h(first), d(first), span(first, last), cudaMemcpyDeviceToHost, st_);
+    return e != cudaSuccess ? e : cudaStreamSynchronize(st_);
 }
 } // namespace svtb200
 

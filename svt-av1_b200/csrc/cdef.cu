@@ -897,10 +897,9 @@ uint64_t cdef_dist_dropin(const void *dst, int hbd, int dstride, const void *src
     const CdefListView *dl = (const CdefListView *)dlist_v;
     // BlockSize: BLOCK_4X4 0, BLOCK_4X8 1, BLOCK_8X4 2, BLOCK_8X8 3
     const int bw = (bsize == 3 || bsize == 2) ? 8 : 4, bh = (bsize == 3 || bsize == 1) ? 8 : 4, n = bw * bh;
-    ThreadCtx &c = tls();
-    const size_t half = ((size_t)count * n * 2 + 15) & ~(size_t)15;
-    c.reserve(2 * half + 16);
-    uint16_t *hd = (uint16_t *)c.h, *hs = (uint16_t *)(c.h + half);
+    Staging s({(size_t)count * n * 2, (size_t)count * n * 2, 8});
+    SVTB_CUDA_FATAL(s.status());
+    uint16_t *hd = s.h<uint16_t>(0), *hs = s.h<uint16_t>(1);
     for (int b = 0; b < count; b++) {
         const int y0 = dl[b].by * bh, x0 = dl[b].bx * bw;
         for (int i = 0; i < bh; i++)
@@ -910,16 +909,12 @@ uint64_t cdef_dist_dropin(const void *dst, int hbd, int dstride, const void *src
                 hs[b * n + i * bw + j] = hbd ? ((const uint16_t *)src)[b * n + i * bw + j] : ((const uint8_t *)src)[b * n + i * bw + j];
             }
     }
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, 2 * half, cudaMemcpyHostToDevice, c.stream));
-    unsigned long long *d_out = (unsigned long long *)(c.d + 2 * half);
-    SVTB_CUDA_FATAL(cudaMemsetAsync(d_out, 0, 8, c.stream));
-    SVTB_LAUNCH(cdef_dist_kernel, 1, 64, 0, c.stream, (const uint16_t *)c.d, (const uint16_t *)(c.d + half), count, bw, bh,
-                (int)(bsize == 3 && pli == 0), coeff_shift, d_out);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h, d_out, 8, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    unsigned long long v;
-    memcpy(&v, c.h, 8);
-    return v >> (2 * coeff_shift);
+    SVTB_CUDA_FATAL(s.upload(0, 1));
+    SVTB_CUDA_FATAL(cudaMemsetAsync(s.d(2), 0, 8, s.stream()));
+    SVTB_LAUNCH(cdef_dist_kernel, 1, 64, 0, s.stream(), s.d<const uint16_t>(0), s.d<const uint16_t>(1), count, bw, bh,
+                (int)(bsize == 3 && pli == 0), coeff_shift, s.d<unsigned long long>(2));
+    SVTB_CUDA_FATAL(s.download(2, 2));
+    return *s.h<unsigned long long>(2) >> (2 * coeff_shift);
 }
 
 __global__ void copy_rect8_kernel(uint16_t *dst, const uint8_t *src, int n) {
@@ -1246,35 +1241,30 @@ int svt_b200_cdef_apply_dev(int32_t mi_rows, int32_t mi_cols, int32_t damping, c
 }
 
 int32_t svt_cdef_find_dir_cuda(const uint16_t *img, int32_t stride, int32_t *var, int32_t coeff_shift) {
-    ThreadCtx &c = tls();
-    c.reserve(256);
-    uint16_t *h = (uint16_t *)c.h;
-    for (int i = 0; i < 8; i++) memcpy(h + 8 * i, img + (size_t)i * stride, 16);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, 128, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(find_dir_kernel, 1, 32, 0, c.stream, (const uint16_t *)c.d, 8, coeff_shift, (int *)(c.d + 128));
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + 128, c.d + 128, 8, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    int r[2];
-    memcpy(r, c.h + 128, 8);
-    *var = r[1];
-    return r[0];
+    Staging s({128, 8});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, img, stride, 2, 8, 8);
+    SVTB_CUDA_FATAL(s.upload(0, 0));
+    SVTB_LAUNCH(find_dir_kernel, 1, 32, 0, s.stream(), s.d<const uint16_t>(0), 8, coeff_shift, s.d<int>(1));
+    SVTB_CUDA_FATAL(s.download(1, 1));
+    *var = s.h<int>(1)[1];
+    return s.h<int>(1)[0];
 }
 
 void svt_cdef_filter_block_cuda(uint8_t *dst8, uint16_t *dst16, int32_t dstride, const uint16_t *in,
                                 int32_t pri_strength, int32_t sec_strength, int32_t dir, int32_t pri_damping,
                                 int32_t sec_damping, int32_t bsize, int32_t coeff_shift) {
     const int rows = 4 << (bsize == 3 || bsize == 1), cols = 4 << (bsize == 3 || bsize == 2);
-    ThreadCtx &c = tls();
-    c.reserve(512);
-    uint16_t *h = (uint16_t *)c.h;
+    Staging s({288, 128}); // the 12x12 window around the block, the 8x8 output
+    SVTB_CUDA_FATAL(s.status());
+    uint16_t *h = s.h<uint16_t>(0);
     for (int i = 0; i < 12; i++)
         for (int j = 0; j < 12; j++) h[i * 12 + j] = (i < rows + 4 && j < cols + 4) ? in[(i - 2) * 144 + (j - 2)] : 0;
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, 288, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(filter_block_kernel, 1, 64, 0, c.stream, (const uint16_t *)c.d, pri_strength, sec_strength, dir,
-                pri_damping, sec_damping, rows, cols, coeff_shift, (uint16_t *)(c.d + 288));
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + 288, c.d + 288, 128, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    const uint16_t *o = (const uint16_t *)(c.h + 288);
+    SVTB_CUDA_FATAL(s.upload(0, 0));
+    SVTB_LAUNCH(filter_block_kernel, 1, 64, 0, s.stream(), s.d<const uint16_t>(0), pri_strength, sec_strength, dir, pri_damping,
+                sec_damping, rows, cols, coeff_shift, s.d<uint16_t>(1));
+    SVTB_CUDA_FATAL(s.download(1, 1));
+    const uint16_t *o = s.h<uint16_t>(1);
     for (int i = 0; i < rows; i++)
         for (int j = 0; j < cols; j++) {
             if (dst8)
@@ -1295,14 +1285,13 @@ uint64_t svt_compute_cdef_dist_8bit_cuda(const uint8_t *dst8, int32_t dstride, c
 
 void svt_copy_rect8_8bit_to_16bit_cuda(uint16_t *dst, int32_t dstride, const uint8_t *src, int32_t sstride, int32_t v, int32_t h) {
     if (v <= 0 || h <= 0) return;
-    ThreadCtx &c = tls();
-    const size_t n = (size_t)v * h, in_b = (n + 15) & ~(size_t)15;
-    c.reserve(in_b + 2 * n);
-    for (int i = 0; i < v; i++) memcpy(c.h + (size_t)i * h, src + (size_t)i * sstride, (size_t)h);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, n, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(copy_rect8_kernel, (int)std::min<size_t>(64, (n + 255) / 256), 256, 0, c.stream, (uint16_t *)(c.d + in_b), (const uint8_t *)c.d, (int)n);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + in_b, c.d + in_b, 2 * n, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    for (int i = 0; i < v; i++) memcpy(dst + (size_t)i * dstride, c.h + in_b + (size_t)i * h * 2, (size_t)h * 2);
+    const size_t n = (size_t)v * h;
+    Staging s({n, 2 * n});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, src, sstride, 1, h, v);
+    SVTB_CUDA_FATAL(s.upload(0, 0));
+    SVTB_LAUNCH(copy_rect8_kernel, (int)std::min<size_t>(64, (n + 255) / 256), 256, 0, s.stream(), s.d<uint16_t>(1), s.d<const uint8_t>(0), (int)n);
+    SVTB_CUDA_FATAL(s.download(1, 1));
+    s.get_rows(1, dst, dstride, 2, h, v);
 }
 }

@@ -1,17 +1,19 @@
 // common.cuh — shared infrastructure of libsvtav1_b200.so (sm_90a only).
 //  * error capture (thread-local message, negative SvtB200Status codes, no CPU fallback)
 //  * launch counter (svt_b200_launch_count)
-//  * ThreadCtx: per-calling-thread stream + growable pinned/device staging for the RTCD drop-ins, which —
-//    like the reference's function pointers (SURVEY §8b) — are re-entrant and called concurrently from
-//    every pipeline thread with raw host pointers.
+//  * Staging: the regions of one host-pointer call in the calling thread's stream + growable pinned/device
+//    buffers.  The RTCD drop-ins — like the reference's function pointers (SURVEY §8b) — are re-entrant and
+//    called concurrently from every pipeline thread with raw host pointers.
 #pragma once
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <cstddef>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 
 #include "../../include/svt_av1_b200.h"
 
@@ -45,15 +47,38 @@ void set_error(const char *fmt, ...);
         if (e__ != cudaSuccess) svtb200::fatal(#expr, e__); \
     } while (0)
 
-struct ThreadCtx {
-    cudaStream_t stream = nullptr;
-    uint8_t *h = nullptr; // pinned
-    uint8_t *d = nullptr; // device
-    size_t cap = 0;
-    int device = -1; // the device stream / d belong to: rebuilt when the calling thread's current device changes
-    void reserve(size_t bytes);
-    void drop();
-    ~ThreadCtx();
+// The staging of one host-pointer call (the RTCD drop-ins and the `_host` entries) on the calling thread's stream and
+// its pinned + device buffers.  A call names its regions in order with their byte sizes; every region starts on a
+// 256-byte boundary, so a kernel that reads a little past the end of its region stays inside the buffers.  The
+// constructor reserves the buffers once, before any region is written; a reservation can move them, so nothing the
+// call runs while it holds region pointers may construct another Staging on the same thread.
+class Staging {
+  public:
+    Staging(std::initializer_list<size_t> region_bytes);
+    // the reservation's error, if any: the thread's buffers are then empty and its next call allocates again
+    cudaError_t status() const { return err_; }
+    cudaStream_t stream() const { return st_; }
+    template <typename T = uint8_t>
+    T *h(int r) const { return reinterpret_cast<T *>(h_ + off_[r]); }
+    template <typename T = uint8_t>
+    T *d(int r) const { return reinterpret_cast<T *>(d_ + off_[r]); }
+    size_t off(int r) const { return off_[r]; }
+    size_t span(int first, int last) const { return off_[last] + bytes_[last] - off_[first]; }
+    // `rows` rows of `width` elements of `es` bytes, `stride` elements apart from `src`, packed into region r
+    void put_rows(int r, const void *src, ptrdiff_t stride, size_t es, size_t width, size_t rows);
+    // the packed rows of region r out to `dst`, `stride` elements apart
+    void get_rows(int r, void *dst, ptrdiff_t stride, size_t es, size_t width, size_t rows) const;
+    // one copy of regions first..last to the device; of the last region only its first `last_bytes`
+    cudaError_t upload(int first, int last, size_t last_bytes = SIZE_MAX);
+    // one copy of regions first..last to the host, then a wait for the stream
+    cudaError_t download(int first, int last);
+
+  private:
+    static constexpr int kMaxRegions = 16;
+    size_t off_[kMaxRegions], bytes_[kMaxRegions];
+    uint8_t *h_ = nullptr, *d_ = nullptr;
+    cudaStream_t st_ = nullptr;
+    cudaError_t err_;
 };
 
 // Per-DEVICE one-time set-up (cudaFuncSetAttribute, occupancy queries and table uploads are per device, a process may
@@ -81,7 +106,6 @@ struct PerDeviceOnce {
     }
 };
 #define SVTB_ATTR(kernel, bytes) SVTB_CUDA_FATAL(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes))
-ThreadCtx &tls();
 
 // ---- device helpers -------------------------------------------------------------------------------
 // 4 byte-wise absolute differences accumulated into acc (PTX vabsdiff4 with the .add merge).

@@ -346,9 +346,9 @@ __global__ void __launch_bounds__(256) sse_kernel(const T *a, int sa, const T *b
 
 void lpf_dropin(void *s, int hbd, int pitch, int vert, int len, const uint8_t *blimit, const uint8_t *limit,
                 const uint8_t *thresh, int bd) {
-    ThreadCtx &c = tls();
-    c.reserve(256);
-    uint16_t *w = (uint16_t *)c.h;
+    Staging st({128}); // 4 lines of 16 samples across the edge
+    SVTB_CUDA_FATAL(st.status());
+    uint16_t *w = st.h<uint16_t>(0);
     const int n = len == 4 ? 2 : len == 6 ? 3 : len == 8 ? 4 : 7;
     const ptrdiff_t across = vert ? 1 : pitch, along = vert ? pitch : 1;
     memset(w, 0, 128);
@@ -358,10 +358,9 @@ void lpf_dropin(void *s, int hbd, int pitch, int vert, int len, const uint8_t *b
             w[i * 16 + 7 - t] = hbd ? ((uint16_t *)s)[op] : ((uint8_t *)s)[op];
             w[i * 16 + 8 + t] = hbd ? ((uint16_t *)s)[oq] : ((uint8_t *)s)[oq];
         }
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, 128, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(lpf_edge_kernel, 1, 32, 0, c.stream, (uint16_t *)c.d, len, (int)*blimit, (int)*limit, (int)*thresh, bd);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h, c.d, 128, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
+    SVTB_CUDA_FATAL(st.upload(0, 0));
+    SVTB_LAUNCH(lpf_edge_kernel, 1, 32, 0, st.stream(), st.d<uint16_t>(0), len, (int)*blimit, (int)*limit, (int)*thresh, bd);
+    SVTB_CUDA_FATAL(st.download(0, 0));
     for (int i = 0; i < 4; i++)
         for (int t = 0; t < n; t++) {
             const ptrdiff_t op = i * along - (t + 1) * across, oq = i * along + t * across;
@@ -512,6 +511,8 @@ struct PickCtx {
     const SvtB200DlfMi *mi;
     uint8_t *d_lut; // device 768 B
     unsigned long long *d_sse; // device
+    uint8_t *h_lut; // pinned staging of the calling thread: the level table, then the SSE read back
+    unsigned long long *h_sse;
     cudaStream_t st;
     int32_t cur[4]; // frame levels as the search progresses (frm_hdr->loop_filter_params)
 };
@@ -534,16 +535,14 @@ int64_t try_filter(PickCtx &c, int level, int plane, int dir) {
     }
     // the trial levels stay in the frame header (set base filters ... :1007-1014)
     for (int i = 0; i < 4; i++) c.cur[i] = lv[i];
-    ThreadCtx &t = tls();
-    t.reserve(1024);
-    uint8_t(*lut)[2][128] = reinterpret_cast<uint8_t(*)[2][128]>(t.h);
+    uint8_t(*lut)[2][128] = reinterpret_cast<uint8_t(*)[2][128]>(c.h_lut);
     svt_b200_lf_level_lut(&c.p->init, lv, lut);
     SvtB200DlfParams dp = c.p->dlf;
     dp.sharpness = 0;
     dp.filter_level[0] = lv[0], dp.filter_level[1] = lv[1], dp.filter_level_u = lv[2], dp.filter_level_v = lv[3];
     dp.plane_start = plane, dp.plane_end = plane + 1;
     // the pinned staging buffer is reused by the next trial: the previous trial ended with a stream synchronise
-    if (cudaMemcpyAsync(c.d_lut, t.h, 768, cudaMemcpyHostToDevice, c.st) != cudaSuccess) return -1;
+    if (cudaMemcpyAsync(c.d_lut, c.h_lut, 768, cudaMemcpyHostToDevice, c.st) != cudaSuccess) return -1;
     if (dlf_frame_impl(&dp, c.recon, c.mi, c.d_lut, c.st) != SVT_B200_OK) return -1;
     if (cudaMemsetAsync(c.d_sse, 0, 8, c.st) != cudaSuccess) return -1;
     const int w = plane ? c.recon->width >> 1 : c.recon->width, h = plane ? c.recon->height >> 1 : c.recon->height;
@@ -556,10 +555,9 @@ int64_t try_filter(PickCtx &c, int level, int plane, int dir) {
     else
         SVTB_LAUNCH(sse_kernel<uint8_t>, grid, 256, 0, c.st, (const uint8_t *)a, sa, (const uint8_t *)b, sb, w, h, c.d_sse);
     if (plane_copy(c.temp, c.recon, plane, c.st)) return -1; // re-instate the unfiltered plane
-    unsigned long long *h_sse = reinterpret_cast<unsigned long long *>(t.h + 768);
-    if (cudaMemcpyAsync(h_sse, c.d_sse, 8, cudaMemcpyDeviceToHost, c.st) != cudaSuccess) return -1;
+    if (cudaMemcpyAsync(c.h_sse, c.d_sse, 8, cudaMemcpyDeviceToHost, c.st) != cudaSuccess) return -1;
     if (cudaStreamSynchronize(c.st) != cudaSuccess) return -1;
-    return (int64_t)*h_sse;
+    return (int64_t)*c.h_sse;
 }
 // search_filter_level (:1027-1191)
 int search_level(PickCtx &c, int plane, int dir, int *err) {
@@ -649,6 +647,11 @@ int svt_b200_pick_filter_level(const SvtB200LpfPickParams *p, const SvtB200Frame
     c.d_lut = (uint8_t *)scratch;
     c.d_sse = (unsigned long long *)((uint8_t *)scratch + 768);
     c.st = (cudaStream_t)stream;
+    // pinned side only, on the caller's stream: reserved once for the whole search (nothing the search runs stages)
+    Staging s({768, 8});
+    SVTB_CUDA_TRY(s.status());
+    c.h_lut = s.h(0);
+    c.h_sse = s.h<unsigned long long>(1);
     for (int i = 0; i < 4; i++) c.cur[i] = p->last_level[i];
     int err = 0;
     const int y = search_level(c, 0, 2, &err);

@@ -449,11 +449,6 @@ __global__ void __launch_bounds__(32) convolve_dropin_kernel(const __grid_consta
     }
 }
 
-template <typename T>
-void gather_rect(T *dst, const T *src, ptrdiff_t stride, int x0, int y0, int w, int h) {
-    for (int y = 0; y < h; y++) memcpy(dst + (size_t)y * w, src + (ptrdiff_t)(y0 + y) * stride + x0, sizeof(T) * (size_t)w);
-}
-
 // `form` = sx * 4 + sy * 2 + compound: which of convolve[sx][sy][is_compound] (:1162-1175) this call is
 template <typename T>
 void convolve_run(const char *name, int form, const T *src, int src_stride, T *dst, int dst_stride, int w, int h,
@@ -465,38 +460,30 @@ void convolve_run(const char *name, int form, const T *src, int src_stride, T *d
         fprintf(stderr, "%s_cuda: bad argument (w %d h %d; 8-tap kernels only)\n", name, w, h);
         abort();
     }
-    ThreadCtx &c = tls();
     const int ww = w + 7, wh = h + 7;
-    const size_t win_b = (sizeof(T) * ww * wh + 15) & ~(size_t)15, conv_b = ((size_t)2 * w * h + 15) & ~(size_t)15;
-    c.reserve(win_b + conv_b + sizeof(T) * w * h);
-    gather_rect<T>((T *)c.h, src, src_stride, -3, -3, ww, wh);
-    size_t up = win_b;
-    if (compound && cp->do_average) {
-        gather_rect<uint16_t>((uint16_t *)(c.h + win_b), cp->dst, cp->dst_stride, 0, 0, w, h);
-        up += conv_b;
-    }
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, up, cudaMemcpyHostToDevice, c.stream));
+    Staging s({sizeof(T) * ww * wh, (size_t)2 * w * h, sizeof(T) * w * h}); // window, conv (compound), out
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, src - 3 * (ptrdiff_t)src_stride - 3, src_stride, sizeof(T), ww, wh);
+    const bool avg = compound && cp->do_average;
+    if (avg) s.put_rows(1, cp->dst, cp->dst_stride, 2, w, h);
+    SVTB_CUDA_FATAL(s.upload(0, avg ? 1 : 0));
     ConvArgs a;
     memset(&a, 0, sizeof(a));
-    a.win = c.d;
-    a.conv = (uint16_t *)(c.d + win_b);
-    a.out = c.d + win_b + conv_b;
+    a.win = s.d(0);
+    a.conv = s.d<uint16_t>(1);
+    a.out = s.d(2);
     a.w = w, a.h = h, a.r0 = cp->round_0, a.r1 = cp->round_1, a.bd = bd;
     a.sx = sx, a.sy = sy, a.compound = compound, a.do_average = cp->do_average;
     a.use_jnt = cp->use_jnt_comp_avg, a.fwd = cp->fwd_offset, a.bck = cp->bck_offset;
     if (sx) memcpy(a.fx, fpx->filter_ptr + 8 * (spx & 15), 16); // av1_get_interp_filter_subpel_kernel
     if (sy) memcpy(a.fy, fpy->filter_ptr + 8 * (spy & 15), 16);
-    SVTB_LAUNCH(convolve_dropin_kernel<T>, dim3((w + TILE_W - 1) / TILE_W, (h + 2 * TILE_H - 1) / (2 * TILE_H)), 32, 0, c.stream, a);
+    SVTB_LAUNCH(convolve_dropin_kernel<T>, dim3((w + TILE_W - 1) / TILE_W, (h + 2 * TILE_H - 1) / (2 * TILE_H)), 32, 0, s.stream(), a);
     const bool to_conv = compound && !cp->do_average;
-    const size_t off = to_conv ? win_b : win_b + conv_b, nb = to_conv ? (size_t)2 * w * h : sizeof(T) * w * h;
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + off, c.d + off, nb, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    for (int y = 0; y < h; y++) {
-        if (to_conv)
-            memcpy(cp->dst + (ptrdiff_t)y * cp->dst_stride, c.h + off + (size_t)2 * y * w, (size_t)2 * w);
-        else
-            memcpy(dst + (ptrdiff_t)y * dst_stride, c.h + off + sizeof(T) * y * w, sizeof(T) * w);
-    }
+    SVTB_CUDA_FATAL(s.download(to_conv ? 1 : 2, to_conv ? 1 : 2));
+    if (to_conv)
+        s.get_rows(1, cp->dst, cp->dst_stride, 2, w, h);
+    else
+        s.get_rows(2, dst, dst_stride, sizeof(T), w, h);
 }
 
 // svt_aom_convolve8_horiz / vert: position q0 + i * step sixteenths along the filtered axis
@@ -535,17 +522,15 @@ void convolve8_run(const uint8_t *src, ptrdiff_t src_stride, uint8_t *dst, ptrdi
     const int span = ((((vert ? h : w) - 1) * step + a.q0) >> 4) + 8; // samples touched along the filtered axis
     const int ww = vert ? w : span, wh = vert ? span : h;
     a.stride = ww;
-    ThreadCtx &c = tls();
-    const size_t win_b = ((size_t)ww * wh + 15) & ~(size_t)15;
-    c.reserve(win_b + (size_t)w * h);
-    gather_rect<uint8_t>(c.h, src, src_stride, vert ? 0 : -3, vert ? -3 : 0, ww, wh);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, win_b, cudaMemcpyHostToDevice, c.stream));
-    a.win = c.d;
-    a.out = c.d + win_b;
-    SVTB_LAUNCH(convolve8_kernel, (w * h + 127) / 128, 128, 0, c.stream, a);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + win_b, c.d + win_b, (size_t)w * h, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    for (int y = 0; y < h; y++) memcpy(dst + (ptrdiff_t)y * dst_stride, c.h + win_b + (size_t)y * w, (size_t)w);
+    Staging s({(size_t)ww * wh, (size_t)w * h});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, vert ? src - 3 * src_stride : src - 3, src_stride, 1, ww, wh);
+    SVTB_CUDA_FATAL(s.upload(0, 0));
+    a.win = s.d(0);
+    a.out = s.d(1);
+    SVTB_LAUNCH(convolve8_kernel, (w * h + 127) / 128, 128, 0, s.stream(), a);
+    SVTB_CUDA_FATAL(s.download(1, 1));
+    s.get_rows(1, dst, dst_stride, 1, w, h);
 }
 
 } // namespace

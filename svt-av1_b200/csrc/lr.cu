@@ -438,20 +438,19 @@ static void sgr_run(const uint8_t *dat8, int width, int height, int stride, int 
         fprintf(stderr, "svt_av1_selfguided_restoration_cuda: unit %dx%d larger than a restoration processing unit\n", width, height);
         abort();
     }
-    ThreadCtx &c = tls();
-    const size_t tile_b = (size_t)(width + 6) * (height + 6) * 2, f_off = (tile_b + 15) & ~(size_t)15,
-                 fb = (size_t)width * height * 4, o_off = f_off + 2 * fb;
-    c.reserve(o_off + (size_t)width * height * 2);
-    gather((uint16_t *)c.h, dat8, highbd, stride, -3, -3, width + 6, height + 6);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, tile_b, cudaMemcpyHostToDevice, c.stream));
+    const size_t tile_b = (size_t)(width + 6) * (height + 6) * 2, fb = (size_t)width * height * 4;
+    Staging s({tile_b, fb, fb, (size_t)width * height * 2});
+    SVTB_CUDA_FATAL(s.status());
+    gather(s.h<uint16_t>(0), dat8, highbd, stride, -3, -3, width + 6, height + 6);
+    SVTB_CUDA_FATAL(s.upload(0, 0));
     SgrArgs a;
-    a.tile_in = (const uint16_t *)c.d;
+    a.tile_in = s.d<const uint16_t>(0);
     a.w = width;
     a.h = height;
     a.bd = bit_depth;
     a.idx = eps;
-    a.flt0 = (int32_t *)(c.d + f_off);
-    a.flt1 = (int32_t *)(c.d + f_off + fb);
+    a.flt0 = s.d<int32_t>(1);
+    a.flt1 = s.d<int32_t>(2);
     a.apply = xqd != nullptr;
     a.xq0 = a.xq1 = 0;
     if (xqd) { // svt_decode_xq
@@ -467,19 +466,15 @@ static void sgr_run(const uint8_t *dat8, int width, int height, int stride, int 
             a.xq1 = 128 - a.xq0 - xqd[1];
         }
     }
-    a.out = (uint16_t *)(c.d + o_off);
+    a.out = s.d<uint16_t>(3);
     const size_t smem = (size_t)2 * (width + 2) * (height + 2) * 4 + tile_b + 16;
-    SVTB_LAUNCH(sgr_kernel, 1, SGR_NT, smem, c.stream, a);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + f_off, c.d + f_off, 2 * fb + (size_t)width * height * 2, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
+    SVTB_LAUNCH(sgr_kernel, 1, SGR_NT, smem, s.stream(), a);
+    SVTB_CUDA_FATAL(s.download(1, 3));
     if (!xqd) {
-        const int32_t *h0 = (const int32_t *)(c.h + f_off), *h1 = (const int32_t *)(c.h + f_off + fb);
-        for (int y = 0; y < height; y++) {
-            if (h_sgr_r[eps][0] > 0) memcpy(flt0 + (size_t)y * flt_stride, h0 + (size_t)y * width, (size_t)width * 4);
-            if (h_sgr_r[eps][1] > 0) memcpy(flt1 + (size_t)y * flt_stride, h1 + (size_t)y * width, (size_t)width * 4);
-        }
+        if (h_sgr_r[eps][0] > 0) s.get_rows(1, flt0, flt_stride, 4, width, height);
+        if (h_sgr_r[eps][1] > 0) s.get_rows(2, flt1, flt_stride, 4, width, height);
     } else {
-        const uint16_t *ho = (const uint16_t *)(c.h + o_off);
+        const uint16_t *ho = s.h<uint16_t>(3);
         for (int y = 0; y < height; y++)
             for (int x = 0; x < width; x++) {
                 if (highbd)
@@ -497,13 +492,13 @@ static void wiener_run(const uint8_t *src, ptrdiff_t src_stride, uint8_t *dst, p
         fprintf(stderr, "svt_av1_wiener_convolve_add_src_cuda: %dx%d out of range\n", w, h);
         abort();
     }
-    ThreadCtx &c = tls();
-    const size_t tile_b = (size_t)(w + 7) * (h + 7) * 2, o_off = (tile_b + 15) & ~(size_t)15;
-    c.reserve(o_off + (size_t)w * h * 2);
-    gather((uint16_t *)c.h, src, highbd, src_stride, -3, -3, w + 7, h + 7);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, tile_b, cudaMemcpyHostToDevice, c.stream));
+    const size_t tile_b = (size_t)(w + 7) * (h + 7) * 2;
+    Staging s({tile_b, (size_t)w * h * 2});
+    SVTB_CUDA_FATAL(s.status());
+    gather(s.h<uint16_t>(0), src, highbd, src_stride, -3, -3, w + 7, h + 7);
+    SVTB_CUDA_FATAL(s.upload(0, 0));
     WienerArgs a;
-    a.tile_in = (const uint16_t *)c.d;
+    a.tile_in = s.d<const uint16_t>(0);
     a.w = w;
     a.h = h;
     a.bd = bd;
@@ -513,12 +508,11 @@ static void wiener_run(const uint8_t *src, ptrdiff_t src_stride, uint8_t *dst, p
     // convolve.c:49-57); with the x/y steps fixed at 16 that always resolves to the 8 taps pointed at
     memcpy(a.fx, filter_x, 16);
     memcpy(a.fy, filter_y, 16);
-    a.out = (uint16_t *)(c.d + o_off);
+    a.out = s.d<uint16_t>(1);
     const size_t smem = tile_b + (size_t)(h + 7) * w * 2 + 16;
-    SVTB_LAUNCH(wiener_kernel, 1, 256, smem, c.stream, a);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + o_off, c.d + o_off, (size_t)w * h * 2, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    const uint16_t *ho = (const uint16_t *)(c.h + o_off);
+    SVTB_LAUNCH(wiener_kernel, 1, 256, smem, s.stream(), a);
+    SVTB_CUDA_FATAL(s.download(1, 1));
+    const uint16_t *ho = s.h<uint16_t>(1);
     for (int y = 0; y < h; y++)
         for (int x = 0; x < w; x++) {
             if (highbd)

@@ -259,35 +259,30 @@ void stats_dropin(int win, const void *dgd, const void *src, int hbd, int h_star
         abort();
     }
     const int es = hbd ? 2 : 1, dw = uw + 2 * hw, dh = uh + 2 * hw;
-    ThreadCtx &c = tls();
-    const size_t dgd_b = ((size_t)dw * dh * es + 15) & ~(size_t)15, src_b = ((size_t)uw * uh * es + 15) & ~(size_t)15;
-    const size_t out_b = (size_t)(win2 + win2 * win2) * 8, tot = dgd_b + src_b + 64 + out_b;
-    c.reserve(tot);
-    for (int y = 0; y < dh; y++)
-        memcpy(c.h + (size_t)y * dw * es, (const uint8_t *)dgd + ((ptrdiff_t)(v_start - hw + y) * dgd_stride + h_start - hw) * es, (size_t)dw * es);
-    for (int y = 0; y < uh; y++)
-        memcpy(c.h + dgd_b + (size_t)y * uw * es, (const uint8_t *)src + ((ptrdiff_t)(v_start + y) * src_stride + h_start) * es, (size_t)uw * es);
-    StatsUnit hu = {hw, hw + uw, hw, hw + uh};
-    memcpy(c.h + dgd_b + src_b, &hu, sizeof(hu));
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, dgd_b + src_b + 16, cudaMemcpyHostToDevice, c.stream));
+    // the unit + halo, the unit's source, then io: StatsUnit at 0, the sum word at 32, M and H from 64
+    Staging s({(size_t)dw * dh * es, (size_t)uw * uh * es, 64 + (size_t)(win2 + win2 * win2) * 8});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, (const uint8_t *)dgd + ((ptrdiff_t)(v_start - hw) * dgd_stride + h_start - hw) * es, dgd_stride, es, dw, dh);
+    s.put_rows(1, (const uint8_t *)src + ((ptrdiff_t)v_start * src_stride + h_start) * es, src_stride, es, uw, uh);
+    *s.h<StatsUnit>(2) = StatsUnit{hw, hw + uw, hw, hw + uh};
+    SVTB_CUDA_FATAL(s.upload(0, 2, sizeof(StatsUnit)));
     StatsDev d;
-    d.dgd = c.d;
-    d.src = c.d + dgd_b - ((size_t)hw * uw + hw) * es; // so that (hw, hw) addresses the first staged source sample
+    d.dgd = s.d(0);
+    d.src = s.d(1) - ((size_t)hw * uw + hw) * es; // so that (hw, hw) addresses the first staged source sample
     d.dgd_stride = dw;
     d.src_stride = uw;
     d.pw = dw;
     d.ph = dh;
     d.clamp = 0;
-    d.units = (const StatsUnit *)(c.d + dgd_b + src_b);
+    d.units = s.d<const StatsUnit>(2);
     d.n_units = 1;
-    d.sum = (unsigned long long *)(c.d + dgd_b + src_b + 32);
-    d.out = (long long *)(c.d + dgd_b + src_b + 64);
+    d.sum = (unsigned long long *)(s.d(2) + 32);
+    d.out = (long long *)(s.d(2) + 64);
     d.divider = !hbd ? 1 : bit_depth == 12 ? 16 : bit_depth == 10 ? 4 : 1;
-    if (stats_launch(d, win, hbd, uw, uh, c.stream)) fatal("svt_av1_compute_stats_cuda", cudaGetLastError());
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h, d.out, out_b, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    memcpy(M, c.h, (size_t)win2 * 8);
-    memcpy(H, c.h + (size_t)win2 * 8, (size_t)win2 * win2 * 8);
+    if (stats_launch(d, win, hbd, uw, uh, s.stream())) fatal("svt_av1_compute_stats_cuda", cudaGetLastError());
+    SVTB_CUDA_FATAL(s.download(2, 2));
+    memcpy(M, s.h(2) + 64, (size_t)win2 * 8);
+    memcpy(H, s.h(2) + 64 + (size_t)win2 * 8, (size_t)win2 * win2 * 8);
 }
 
 // ---- pixel projection error -----------------------------------------------------------------------------------
@@ -319,36 +314,40 @@ __global__ void __launch_bounds__(256) proj_error_kernel(const ProjArgs a) {
     if ((threadIdx.x & 31) == 0 && acc) atomicAdd(a.out, (unsigned long long)acc);
 }
 
+// the staging of both projection drop-ins: src, dat and the filtered planes the parameters use packed and uploaded,
+// then region 4 (= a.out): n_out 64-bit sums, zeroed on the device
+Staging proj_stage(ProjArgs &a, const void *src, int width, int height, int src_stride, const void *dat, int dat_stride,
+                   const int32_t *flt0, int f0s, const int32_t *flt1, int f1s, const int32_t *params, int hbd, int n_out) {
+    const int es = hbd ? 2 : 1, r0 = params[0], r1 = params[1];
+    const size_t pb = (size_t)width * height * es, fb = (size_t)width * height * 4;
+    Staging s({pb, pb, fb, fb, (size_t)n_out * 8});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, src, src_stride, es, width, height);
+    s.put_rows(1, dat, dat_stride, es, width, height);
+    if (r0 > 0) s.put_rows(2, flt0, f0s, 4, width, height);
+    if (r1 > 0) s.put_rows(3, flt1, f1s, 4, width, height);
+    SVTB_CUDA_FATAL(s.upload(0, 3));
+    a.src = s.d(0);
+    a.dat = s.d(1);
+    a.flt0 = s.d<const int32_t>(2);
+    a.flt1 = s.d<const int32_t>(3);
+    a.w = width, a.h = height, a.src_stride = a.dat_stride = a.f0s = a.f1s = width;
+    a.xq0 = a.xq1 = 0, a.r0 = r0, a.r1 = r1, a.hbd = hbd;
+    a.out = s.d<unsigned long long>(4);
+    SVTB_CUDA_FATAL(cudaMemsetAsync(a.out, 0, (size_t)n_out * 8, s.stream()));
+    return s;
+}
+
 int64_t proj_dropin(const void *src, int width, int height, int src_stride, const void *dat, int dat_stride, const int32_t *flt0,
                     int f0s, const int32_t *flt1, int f1s, const int32_t *xq, const int32_t *params /* SgrParamsType: r[2], s[2] */,
                     int hbd) {
     if (width <= 0 || height <= 0) return 0;
-    const int es = hbd ? 2 : 1, r0 = params[0], r1 = params[1];
-    ThreadCtx &c = tls();
-    const size_t pb = ((size_t)width * height * es + 15) & ~(size_t)15, fb = (size_t)width * height * 4;
-    c.reserve(2 * pb + 2 * fb + 16);
-    for (int y = 0; y < height; y++) {
-        memcpy(c.h + (size_t)y * width * es, (const uint8_t *)src + (size_t)y * src_stride * es, (size_t)width * es);
-        memcpy(c.h + pb + (size_t)y * width * es, (const uint8_t *)dat + (size_t)y * dat_stride * es, (size_t)width * es);
-        if (r0 > 0) memcpy(c.h + 2 * pb + (size_t)y * width * 4, flt0 + (size_t)y * f0s, (size_t)width * 4);
-        if (r1 > 0) memcpy(c.h + 2 * pb + fb + (size_t)y * width * 4, flt1 + (size_t)y * f1s, (size_t)width * 4);
-    }
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, 2 * pb + 2 * fb, cudaMemcpyHostToDevice, c.stream));
     ProjArgs a;
-    a.src = c.d;
-    a.dat = c.d + pb;
-    a.flt0 = (const int32_t *)(c.d + 2 * pb);
-    a.flt1 = (const int32_t *)(c.d + 2 * pb + fb);
-    a.w = width, a.h = height, a.src_stride = a.dat_stride = a.f0s = a.f1s = width;
-    a.xq0 = xq[0], a.xq1 = xq[1], a.r0 = r0, a.r1 = r1, a.hbd = hbd;
-    a.out = (unsigned long long *)(c.d + 2 * pb + 2 * fb);
-    SVTB_CUDA_FATAL(cudaMemsetAsync(a.out, 0, 8, c.stream));
-    SVTB_LAUNCH(proj_error_kernel, std::min(64, (width * height + 255) / 256), 256, 0, c.stream, a);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h, a.out, 8, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    int64_t v;
-    memcpy(&v, c.h, 8);
-    return v;
+    Staging s = proj_stage(a, src, width, height, src_stride, dat, dat_stride, flt0, f0s, flt1, f1s, params, hbd, 1);
+    a.xq0 = xq[0], a.xq1 = xq[1];
+    SVTB_LAUNCH(proj_error_kernel, std::min(64, (width * height + 255) / 256), 256, 0, s.stream(), a);
+    SVTB_CUDA_FATAL(s.download(4, 4));
+    return *s.h<int64_t>(4);
 }
 
 // svt_get_proj_subspace_c (EbRestorationPick.c:337-440): the five sums over the unit.  The reference accumulates them
@@ -377,32 +376,13 @@ void proj_subspace_dropin(const void *src, int width, int height, int src_stride
                           const int32_t *flt0, int f0s, const int32_t *flt1, int f1s, int *xq, const int32_t *params) {
     xq[0] = xq[1] = 0;
     if (width <= 0 || height <= 0) return;
-    const int es = hbd ? 2 : 1, r0 = params[0], r1 = params[1];
-    ThreadCtx &c = tls();
-    const size_t pb = ((size_t)width * height * es + 15) & ~(size_t)15, fb = (size_t)width * height * 4;
-    c.reserve(2 * pb + 2 * fb + 64);
-    for (int y = 0; y < height; y++) {
-        memcpy(c.h + (size_t)y * width * es, (const uint8_t *)src + (size_t)y * src_stride * es, (size_t)width * es);
-        memcpy(c.h + pb + (size_t)y * width * es, (const uint8_t *)dat + (size_t)y * dat_stride * es, (size_t)width * es);
-        if (r0 > 0) memcpy(c.h + 2 * pb + (size_t)y * width * 4, flt0 + (size_t)y * f0s, (size_t)width * 4);
-        if (r1 > 0) memcpy(c.h + 2 * pb + fb + (size_t)y * width * 4, flt1 + (size_t)y * f1s, (size_t)width * 4);
-    }
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, 2 * pb + 2 * fb, cudaMemcpyHostToDevice, c.stream));
+    const int r0 = params[0], r1 = params[1];
     ProjArgs a;
-    a.src = c.d;
-    a.dat = c.d + pb;
-    a.flt0 = (const int32_t *)(c.d + 2 * pb);
-    a.flt1 = (const int32_t *)(c.d + 2 * pb + fb);
-    a.w = width, a.h = height, a.src_stride = a.dat_stride = a.f0s = a.f1s = width;
-    a.xq0 = a.xq1 = 0, a.r0 = r0, a.r1 = r1, a.hbd = hbd;
-    a.out = nullptr;
-    long long *d_out = (long long *)(c.d + 2 * pb + 2 * fb);
-    SVTB_CUDA_FATAL(cudaMemsetAsync(d_out, 0, 40, c.stream));
-    SVTB_LAUNCH(proj_sums_kernel, std::min(64, (width * height + 255) / 256), 256, 0, c.stream, a, d_out);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h, d_out, 40, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
+    Staging s = proj_stage(a, src, width, height, src_stride, dat, dat_stride, flt0, f0s, flt1, f1s, params, hbd, 5);
+    SVTB_LAUNCH(proj_sums_kernel, std::min(64, (width * height + 255) / 256), 256, 0, s.stream(), a, s.d<long long>(4));
+    SVTB_CUDA_FATAL(s.download(4, 4));
     long long v[5];
-    memcpy(v, c.h, 40);
+    memcpy(v, s.h(4), 40);
     const int size = width * height;
     double H[2][2], C[2], det, x[2];
     H[0][0] = (double)v[0], H[1][1] = (double)v[1], H[0][1] = (double)v[2], C[0] = (double)v[3], C[1] = (double)v[4];

@@ -1360,16 +1360,6 @@ __global__ void ext_sad_32_64_kernel(uint32_t mv, uint32_t *io) {
     }
 }
 
-__global__ void nxm_sad_kernel(const uint8_t *src, int ss, const uint8_t *ref, int rs, int h, int w, uint32_t *out) {
-    uint32_t v = 0;
-    for (int i = threadIdx.x; i < h * w; i += blockDim.x) {
-        int y = i / w, x = i - y * w;
-        v += abs((int)src[(size_t)y * ss + x] - (int)ref[(size_t)y * rs + x]);
-    }
-    v = __reduce_add_sync(0xffffffffu, v);
-    if ((threadIdx.x & 31) == 0) atomicAdd(out, v);
-}
-
 __global__ void fill32_kernel(uint32_t *p, int n, uint32_t v) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) p[i] = v;
@@ -1384,11 +1374,6 @@ static void set_attrs() {
         SVTB_ATTR(fullpel_kernel<false>, FP_SMEM_BYTES);
         SVTB_ATTR(sad_loop_kernel, 200 * 1024);
     });
-}
-
-// copy a w x h byte rectangle (row stride `stride`) into a tight buffer
-static void pack_rect(uint8_t *dst, const uint8_t *src, size_t stride, int w, int h) {
-    for (int y = 0; y < h; y++) memcpy(dst + (size_t)y * w, src + (size_t)y * stride, w);
 }
 
 } // namespace
@@ -1549,16 +1534,14 @@ void svt_sad_loop_kernel_cuda(uint8_t *src, uint32_t src_stride, uint8_t *ref, u
     const int k = ref_stride / src_stride_raw;
     const int bw = block_width, bh = block_height, saw = search_area_width, sah = search_area_height;
     const int ww = saw - 1 + bw, wh = (sah - 1) + (bh - 1) * k + 1;
-    const size_t src_bytes = (size_t)bw * bh, win_bytes = (size_t)ww * wh;
-    const size_t off_win = (src_bytes + 15) & ~(size_t)15, off_out = (off_win + win_bytes + 15) & ~(size_t)15;
-    ThreadCtx &c = tls();
-    c.reserve(off_out + 16);
-    pack_rect(c.h, src, src_stride, bw, bh);
-    pack_rect(c.h + off_win, ref, src_stride_raw, ww, wh);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, off_out, cudaMemcpyHostToDevice, c.stream));
+    Staging s({(size_t)bw * bh, (size_t)ww * wh, 8});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, src, src_stride, 1, bw, bh);
+    s.put_rows(1, ref, src_stride_raw, 1, ww, wh);
+    SVTB_CUDA_FATAL(s.upload(0, 1));
     SadLoopArgs a;
-    a.src = c.d;
-    a.ref = c.d + off_win;
+    a.src = s.d(0);
+    a.ref = s.d(1);
     a.src_stride = bw;
     a.raw_stride = ww;
     a.k = k;
@@ -1566,7 +1549,7 @@ void svt_sad_loop_kernel_cuda(uint8_t *src, uint32_t src_stride, uint8_t *ref, u
     a.bh = bh;
     a.saw = saw;
     a.sah = sah;
-    a.out = (uint64_t *)(c.d + off_out);
+    a.out = s.d<uint64_t>(2);
     // enough shared memory for the source block + at least one search row, up to 200 KB
     const size_t spw = (bw + 3) / 4, wpw = (ww + 3) / 4 + 1;
     size_t need = spw * bh * 4 + wpw * 4 * (size_t)wh;
@@ -1577,11 +1560,9 @@ void svt_sad_loop_kernel_cuda(uint8_t *src, uint32_t src_stride, uint8_t *ref, u
     }
     if (need > 200 * 1024) need = 200 * 1024;
     a.smem_bytes = (int)need;
-    SVTB_LAUNCH(sad_loop_kernel, 1, NT_SEARCH, need, c.stream, a);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + off_out, c.d + off_out, 8, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    uint64_t key;
-    memcpy(&key, c.h + off_out, 8);
+    SVTB_LAUNCH(sad_loop_kernel, 1, NT_SEARCH, need, s.stream(), a);
+    SVTB_CUDA_FATAL(s.download(2, 2));
+    const uint64_t key = *s.h<uint64_t>(2);
     const uint32_t sad = (uint32_t)(key >> 32), idx = (uint32_t)key;
     if (sad < 0xffffffu) { // strict < against the 0xffffff start value
         *best_sad = sad;
@@ -1595,21 +1576,18 @@ void svt_ext_all_sad_calculation_8x8_16x16_cuda(uint8_t *src, uint32_t src_strid
                                                 uint32_t *p_best_sad_16x16, uint32_t *p_best_mv8x8,
                                                 uint32_t *p_best_mv16x16, uint32_t p_eight_sad16x16[16][8],
                                                 uint32_t p_eight_sad8x8[64][8], uint8_t sub_sad) {
-    ThreadCtx &c = tls();
-    const size_t off_ref = 64 * 64, off_io = off_ref + 72 * 64, total = off_io + 800 * 4;
-    c.reserve(total);
-    pack_rect(c.h, src, src_stride, 64, 64);
-    pack_rect(c.h + off_ref, ref, ref_stride, 71, 64);
-    uint32_t *io = (uint32_t *)(c.h + off_io);
+    Staging s({64 * 64, 71 * 64, 800 * 4});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, src, src_stride, 1, 64, 64);
+    s.put_rows(1, ref, ref_stride, 1, 71, 64);
+    uint32_t *io = s.h<uint32_t>(2);
     memcpy(io, p_best_sad_8x8, 64 * 4);
     memcpy(io + 64, p_best_sad_16x16, 16 * 4);
     memcpy(io + 80, p_best_mv8x8, 64 * 4);
     memcpy(io + 144, p_best_mv16x16, 16 * 4);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, off_io + 160 * 4, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(ext_all_sad_kernel, 1, 128, 0, c.stream, c.d, 64, c.d + off_ref, 71, mv, (int)sub_sad,
-                (uint32_t *)(c.d + off_io));
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + off_io, c.d + off_io, 800 * 4, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
+    SVTB_CUDA_FATAL(s.upload(0, 2, 160 * 4));
+    SVTB_LAUNCH(ext_all_sad_kernel, 1, 128, 0, s.stream(), s.d(0), 64, s.d(1), 71, mv, (int)sub_sad, s.d<uint32_t>(2));
+    SVTB_CUDA_FATAL(s.download(2, 2));
     memcpy(p_best_sad_8x8, io, 64 * 4);
     memcpy(p_best_sad_16x16, io + 64, 16 * 4);
     memcpy(p_best_mv8x8, io + 80, 64 * 4);
@@ -1622,18 +1600,17 @@ void svt_ext_eight_sad_calculation_32x32_64x64_cuda(uint32_t p_sad16x16[16][8], 
                                                     uint32_t *p_best_sad_64x64, uint32_t *p_best_mv32x32,
                                                     uint32_t *p_best_mv64x64, uint32_t mv,
                                                     uint32_t p_sad32x32[4][8]) {
-    ThreadCtx &c = tls();
-    c.reserve(170 * 4);
-    uint32_t *io = (uint32_t *)c.h;
+    Staging s({170 * 4});
+    SVTB_CUDA_FATAL(s.status());
+    uint32_t *io = s.h<uint32_t>(0);
     memcpy(io, p_sad16x16, 128 * 4);
     memcpy(io + 128, p_best_sad_32x32, 16);
     io[132] = *p_best_sad_64x64;
     memcpy(io + 133, p_best_mv32x32, 16);
     io[137] = *p_best_mv64x64;
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, 138 * 4, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(ext_eight_32_64_kernel, 1, 32, 0, c.stream, mv, (uint32_t *)c.d);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h, c.d, 170 * 4, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
+    SVTB_CUDA_FATAL(s.upload(0, 0, 138 * 4));
+    SVTB_LAUNCH(ext_eight_32_64_kernel, 1, 32, 0, s.stream(), mv, s.d<uint32_t>(0));
+    SVTB_CUDA_FATAL(s.download(0, 0));
     memcpy(p_best_sad_32x32, io + 128, 16);
     *p_best_sad_64x64 = io[132];
     memcpy(p_best_mv32x32, io + 133, 16);
@@ -1645,21 +1622,18 @@ void svt_ext_sad_calculation_8x8_16x16_cuda(uint8_t *src, uint32_t src_stride, u
                                             uint32_t *p_best_sad_8x8, uint32_t *p_best_sad_16x16,
                                             uint32_t *p_best_mv8x8, uint32_t *p_best_mv16x16, uint32_t mv,
                                             uint32_t *p_sad16x16, uint32_t *p_sad8x8, uint8_t sub_sad) {
-    ThreadCtx &c = tls();
-    const size_t off_ref = 256, off_io = 512;
-    c.reserve(off_io + 64);
-    pack_rect(c.h, src, src_stride, 16, 16);
-    pack_rect(c.h + off_ref, ref, ref_stride, 16, 16);
-    uint32_t *io = (uint32_t *)(c.h + off_io);
+    Staging s({256, 256, 15 * 4});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, src, src_stride, 1, 16, 16);
+    s.put_rows(1, ref, ref_stride, 1, 16, 16);
+    uint32_t *io = s.h<uint32_t>(2);
     memcpy(io, p_best_sad_8x8, 16);
     io[4] = *p_best_sad_16x16;
     memcpy(io + 5, p_best_mv8x8, 16);
     io[9] = *p_best_mv16x16;
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, off_io + 40, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(ext_sad_8_16_kernel, 1, 32, 0, c.stream, c.d, 16, c.d + off_ref, 16, mv, (int)sub_sad,
-                (uint32_t *)(c.d + off_io));
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + off_io, c.d + off_io, 60, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
+    SVTB_CUDA_FATAL(s.upload(0, 2, 10 * 4));
+    SVTB_LAUNCH(ext_sad_8_16_kernel, 1, 32, 0, s.stream(), s.d(0), 16, s.d(1), 16, mv, (int)sub_sad, s.d<uint32_t>(2));
+    SVTB_CUDA_FATAL(s.download(2, 2));
     memcpy(p_best_sad_8x8, io, 16);
     *p_best_sad_16x16 = io[4];
     memcpy(p_best_mv8x8, io + 5, 16);
@@ -1671,18 +1645,17 @@ void svt_ext_sad_calculation_8x8_16x16_cuda(uint8_t *src, uint32_t src_stride, u
 void svt_ext_sad_calculation_32x32_64x64_cuda(uint32_t *p_sad16x16, uint32_t *p_best_sad_32x32,
                                               uint32_t *p_best_sad_64x64, uint32_t *p_best_mv32x32,
                                               uint32_t *p_best_mv64x64, uint32_t mv, uint32_t *p_sad32x32) {
-    ThreadCtx &c = tls();
-    c.reserve(128);
-    uint32_t *io = (uint32_t *)c.h;
+    Staging s({30 * 4});
+    SVTB_CUDA_FATAL(s.status());
+    uint32_t *io = s.h<uint32_t>(0);
     memcpy(io, p_sad16x16, 64);
     memcpy(io + 16, p_best_sad_32x32, 16);
     io[20] = *p_best_sad_64x64;
     memcpy(io + 21, p_best_mv32x32, 16);
     io[25] = *p_best_mv64x64;
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, 26 * 4, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(ext_sad_32_64_kernel, 1, 32, 0, c.stream, mv, (uint32_t *)c.d);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h, c.d, 30 * 4, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
+    SVTB_CUDA_FATAL(s.upload(0, 0, 26 * 4));
+    SVTB_LAUNCH(ext_sad_32_64_kernel, 1, 32, 0, s.stream(), mv, s.d<uint32_t>(0));
+    SVTB_CUDA_FATAL(s.download(0, 0));
     memcpy(p_best_sad_32x32, io + 16, 16);
     *p_best_sad_64x64 = io[20];
     memcpy(p_best_mv32x32, io + 21, 16);
@@ -1690,33 +1663,13 @@ void svt_ext_sad_calculation_32x32_64x64_cuda(uint32_t *p_sad16x16, uint32_t *p_
     memcpy(p_sad32x32, io + 26, 16);
 }
 
-uint32_t svt_nxm_sad_kernel_cuda(const uint8_t *src, uint32_t src_stride, const uint8_t *ref, uint32_t ref_stride,
-                                 uint32_t height, uint32_t width) {
-    if (!height || !width) return 0;
-    ThreadCtx &c = tls();
-    const size_t n = (size_t)width * height, off_ref = (n + 15) & ~(size_t)15, off_out = 2 * off_ref;
-    c.reserve(off_out + 16);
-    pack_rect(c.h, src, src_stride, width, height);
-    pack_rect(c.h + off_ref, ref, ref_stride, width, height);
-    memset(c.h + off_out, 0, 4);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, off_out + 4, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(nxm_sad_kernel, 1, 256, 0, c.stream, c.d, (int)width, c.d + off_ref, (int)width, (int)height,
-                (int)width, (uint32_t *)(c.d + off_out));
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + off_out, c.d + off_out, 4, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    uint32_t v;
-    memcpy(&v, c.h + off_out, 4);
-    return v;
-}
-
 void svt_initialize_buffer_32bits_cuda(uint32_t *pointer, uint32_t count128, uint32_t count32, uint32_t value) {
     const int n = (int)(count128 * 4 + count32);
     if (n <= 0) return;
-    ThreadCtx &c = tls();
-    c.reserve((size_t)n * 4);
-    SVTB_LAUNCH(fill32_kernel, (n + 255) / 256, 256, 0, c.stream, (uint32_t *)c.d, n, value);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h, c.d, (size_t)n * 4, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    memcpy(pointer, c.h, (size_t)n * 4);
+    Staging s({(size_t)n * 4});
+    SVTB_CUDA_FATAL(s.status());
+    SVTB_LAUNCH(fill32_kernel, (n + 255) / 256, 256, 0, s.stream(), s.d<uint32_t>(0), n, value);
+    SVTB_CUDA_FATAL(s.download(0, 0));
+    memcpy(pointer, s.h(0), (size_t)n * 4);
 }
 }

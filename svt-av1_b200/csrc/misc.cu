@@ -4,7 +4,7 @@
 //   svt_full_distortion_kernel32_bits / _cbf_zero32_bits            Common/Codec/EbPictureOperators.c:156-231
 //   svt_spatial_full_distortion_kernel / svt_full_distortion_kernel16_bits  Common/C_DEFAULT/EbPictureOperators_C.c:65, EbPictureOperators.c:182
 //   svt_aom_satd, svt_av1_block_error                               Common/Codec/common_dsp_rtcd.c:47-69
-//   svt_aom_sadMxN, svt_aom_sadMxNx4d (22 sizes), svt_nxm_sad_kernel_sub_sampled, sad_16b_kernel
+//   svt_aom_sadMxN, svt_aom_sadMxNx4d (22 sizes), svt_nxm_sad_kernel(_sub_sampled), sad_16b_kernel
 //                                                                   Encoder/C_DEFAULT/sad_av1.c, EbComputeSAD_C.c:39-56
 // One block-wide reduction kernel serves all of them (mode selects the per-element term); these calls are tiny, so
 // the wrappers exist for pointer-table completeness and parity tests, not for throughput.
@@ -73,43 +73,37 @@ __global__ void subtract_kernel(const T *src, const T *pred, int16_t *diff, int 
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) diff[i] = (int16_t)((int)src[i] - (int)pred[i]);
 }
 
-static void pack(uint8_t *dst, const void *src, size_t stride_elems, int w, int h, int esz) {
-    for (int y = 0; y < h; y++) memcpy(dst + (size_t)y * w * esz, (const uint8_t *)src + (size_t)y * stride_elems * esz, (size_t)w * esz);
-}
-
 // returns {r0, r1}
 static void reduce2(const void *a, size_t sa, const void *b, size_t sb, int w, int h, int esz, int mode, uint64_t res[2]) {
-    ThreadCtx &c = tls();
-    const size_t nb = (size_t)w * h * esz, off_b = (nb + 15) & ~(size_t)15, off_o = 2 * off_b;
-    c.reserve(off_o + 16);
-    pack(c.h, a, sa, w, h, esz);
-    if (b) pack(c.h + off_b, b, sb, w, h, esz);
-    memset(c.h + off_o, 0, 16);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, off_o + 16, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(reduce2_kernel, 1, 256, 0, c.stream, (const void *)c.d, (const void *)(c.d + off_b), w * h, mode,
-                (unsigned long long *)(c.d + off_o));
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + off_o, c.d + off_o, 16, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    memcpy(res, c.h + off_o, 16);
+    const size_t nb = (size_t)w * h * esz;
+    Staging s({nb, nb, 16});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, a, sa, esz, w, h);
+    if (b) s.put_rows(1, b, sb, esz, w, h);
+    memset(s.h(2), 0, 16);
+    SVTB_CUDA_FATAL(s.upload(0, 2));
+    SVTB_LAUNCH(reduce2_kernel, 1, 256, 0, s.stream(), (const void *)s.d(0), (const void *)s.d(1), w * h, mode,
+                s.d<unsigned long long>(2));
+    SVTB_CUDA_FATAL(s.download(2, 2));
+    memcpy(res, s.h(2), 16);
 }
 
 static void subtract(int rows, int cols, int16_t *diff, ptrdiff_t ds, const void *src, ptrdiff_t ss, const void *pred, ptrdiff_t ps,
                      int esz) {
-    ThreadCtx &c = tls();
-    const size_t nb = (size_t)rows * cols * esz, off_p = (nb + 15) & ~(size_t)15, off_d = 2 * off_p;
-    c.reserve(off_d + (size_t)rows * cols * 2);
-    pack(c.h, src, ss, cols, rows, esz);
-    pack(c.h + off_p, pred, ps, cols, rows, esz);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, off_d, cudaMemcpyHostToDevice, c.stream));
+    const size_t nb = (size_t)rows * cols * esz;
+    Staging s({nb, nb, (size_t)rows * cols * 2});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, src, ss, esz, cols, rows);
+    s.put_rows(1, pred, ps, esz, cols, rows);
+    SVTB_CUDA_FATAL(s.upload(0, 1));
     if (esz == 2)
-        SVTB_LAUNCH(subtract_kernel<uint16_t>, 4, 256, 0, c.stream, (const uint16_t *)c.d, (const uint16_t *)(c.d + off_p),
-                    (int16_t *)(c.d + off_d), rows * cols);
+        SVTB_LAUNCH(subtract_kernel<uint16_t>, 4, 256, 0, s.stream(), s.d<const uint16_t>(0), s.d<const uint16_t>(1), s.d<int16_t>(2),
+                    rows * cols);
     else
-        SVTB_LAUNCH(subtract_kernel<uint8_t>, 4, 256, 0, c.stream, (const uint8_t *)c.d, (const uint8_t *)(c.d + off_p),
-                    (int16_t *)(c.d + off_d), rows * cols);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + off_d, c.d + off_d, (size_t)rows * cols * 2, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    for (int y = 0; y < rows; y++) memcpy(diff + (ptrdiff_t)y * ds, c.h + off_d + (size_t)y * cols * 2, (size_t)cols * 2);
+        SVTB_LAUNCH(subtract_kernel<uint8_t>, 4, 256, 0, s.stream(), s.d<const uint8_t>(0), s.d<const uint8_t>(1), s.d<int16_t>(2),
+                    rows * cols);
+    SVTB_CUDA_FATAL(s.download(2, 2));
+    s.get_rows(2, diff, ds, 2, cols, rows);
 }
 
 } // namespace
@@ -161,6 +155,13 @@ int64_t svt_av1_block_error_cuda(const int32_t *coeff, const int32_t *dqcoeff, i
     reduce2(coeff, block_size, dqcoeff, block_size, (int)block_size, 1, 4, M_BLKERR, r);
     *ssz = (int64_t)r[1];
     return (int64_t)r[0];
+}
+uint32_t svt_nxm_sad_kernel_cuda(const uint8_t *src, uint32_t src_stride, const uint8_t *ref, uint32_t ref_stride, uint32_t height,
+                                 uint32_t width) {
+    if (!height || !width) return 0;
+    uint64_t r[2];
+    reduce2(src, src_stride, ref, ref_stride, width, height, 1, M_SAD8, r);
+    return (uint32_t)r[0];
 }
 uint32_t svt_nxm_sad_kernel_sub_sampled_cuda(const uint8_t *src, uint32_t src_stride, const uint8_t *ref, uint32_t ref_stride,
                                              uint32_t height, uint32_t width) {

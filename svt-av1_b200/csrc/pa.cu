@@ -142,32 +142,28 @@ int svt_b200_picture_mean_variance_host(const uint8_t *y, int32_t stride_y, cons
         return SVT_B200_ERR_ARG;
     }
     const int cw = (width + 1) >> 1, ch = (height + 1) >> 1, n_sb = ((width + 63) / 64) * ((height + 63) / 64);
-    auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    const size_t o_y = 0, o_cb = al((size_t)width * height), o_cr = o_cb + al((size_t)cw * ch), o_out = o_cr + al((size_t)cw * ch);
-    const size_t o_var = o_out + al((size_t)n_sb * 85), o_cbm = o_var + al((size_t)n_sb * 170), o_crm = o_cbm + al((size_t)n_sb * 21);
-    const size_t o_avg = o_crm + al((size_t)n_sb * 21), total = o_avg + 256;
-    ThreadCtx &c = tls();
-    c.reserve(total);
-    for (int r = 0; r < height; r++) memcpy(c.h + o_y + (size_t)r * width, y + (size_t)r * stride_y, width);
-    if (cb_mean)
-        for (int r = 0; r < ch; r++) {
-            memcpy(c.h + o_cb + (size_t)r * cw, cb + (size_t)r * stride_c, cw);
-            memcpy(c.h + o_cr + (size_t)r * cw, cr + (size_t)r * stride_c, cw);
-        }
-    SVTB_CUDA_TRY(cudaMemcpyAsync(c.d, c.h, cb_mean ? o_out : o_cb, cudaMemcpyHostToDevice, c.stream));
-    SvtB200Frame f = {c.d + o_y, cb_mean ? c.d + o_cb : nullptr, cb_mean ? c.d + o_cr : nullptr, width, cw, width, height, 8};
-    const int rc = svt_b200_picture_mean_variance(&f, 0, c.d + o_out, (uint16_t *)(c.d + o_var), cb_mean ? c.d + o_cbm : nullptr,
-                                                  cb_mean ? c.d + o_crm : nullptr, (uint16_t *)(c.d + o_avg), c.d + o_avg + 64, c.stream);
-    if (rc) return rc;
-    SVTB_CUDA_TRY(cudaMemcpyAsync(c.h + o_out, c.d + o_out, total - o_out, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_TRY(cudaStreamSynchronize(c.stream));
-    memcpy(y_mean, c.h + o_out, (size_t)n_sb * 85);
-    memcpy(variance, c.h + o_var, (size_t)n_sb * 170);
+    // y | cb | cr in; y mean | variance | cb mean | cr mean | (average variance, its 8-byte sum at 64) out
+    Staging s({(size_t)width * height, (size_t)cw * ch, (size_t)cw * ch, (size_t)n_sb * 85, (size_t)n_sb * 170, (size_t)n_sb * 21,
+               (size_t)n_sb * 21, 72});
+    SVTB_CUDA_TRY(s.status());
+    s.put_rows(0, y, stride_y, 1, width, height);
     if (cb_mean) {
-        memcpy(cb_mean, c.h + o_cbm, (size_t)n_sb * 21);
-        memcpy(cr_mean, c.h + o_crm, (size_t)n_sb * 21);
+        s.put_rows(1, cb, stride_c, 1, cw, ch);
+        s.put_rows(2, cr, stride_c, 1, cw, ch);
     }
-    if (pic_avg_variance) memcpy(pic_avg_variance, c.h + o_avg, 2);
+    SVTB_CUDA_TRY(s.upload(0, cb_mean ? 2 : 0));
+    SvtB200Frame f = {s.d(0), cb_mean ? s.d(1) : nullptr, cb_mean ? s.d(2) : nullptr, width, cw, width, height, 8};
+    const int rc = svt_b200_picture_mean_variance(&f, 0, s.d(3), s.d<uint16_t>(4), cb_mean ? s.d(5) : nullptr, cb_mean ? s.d(6) : nullptr,
+                                                  s.d<uint16_t>(7), s.d(7) + 64, s.stream());
+    if (rc) return rc;
+    SVTB_CUDA_TRY(s.download(3, 7));
+    memcpy(y_mean, s.h(3), (size_t)n_sb * 85);
+    memcpy(variance, s.h(4), (size_t)n_sb * 170);
+    if (cb_mean) {
+        memcpy(cb_mean, s.h(5), (size_t)n_sb * 21);
+        memcpy(cr_mean, s.h(6), (size_t)n_sb * 21);
+    }
+    if (pic_avg_variance) memcpy(pic_avg_variance, s.h(7), 2);
     return SVT_B200_OK;
 }
 }

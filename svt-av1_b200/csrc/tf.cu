@@ -271,14 +271,13 @@ int svt_b200_tf_normalize(const SvtB200Frame *dst, const SvtB200TfAccum *acc, in
 
 // checksum of this library's expf over the floats with bit patterns lo..hi (test hook: compared with the oracle's)
 int svt_b200_tf_expf_checksum(uint32_t lo_bits, uint32_t hi_bits, uint64_t *out_host) {
-    ThreadCtx &c = tls();
-    c.reserve(64);
-    SVTB_CUDA_TRY(cudaMemsetAsync(c.d, 0, 8, c.stream));
-    expf_checksum_kernel<<<132 * 8, 256, 0, c.stream>>>(lo_bits, hi_bits, reinterpret_cast<unsigned long long *>(c.d));
+    Staging s({8});
+    SVTB_CUDA_TRY(s.status());
+    SVTB_CUDA_TRY(cudaMemsetAsync(s.d(0), 0, 8, s.stream()));
+    SVTB_LAUNCH(expf_checksum_kernel, 132 * 8, 256, 0, s.stream(), lo_bits, hi_bits, s.d<unsigned long long>(0));
     SVTB_CUDA_TRY(cudaGetLastError());
-    SVTB_CUDA_TRY(cudaMemcpyAsync(c.h, c.d, 8, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_TRY(cudaStreamSynchronize(c.stream));
-    memcpy(out_host, c.h, 8);
+    SVTB_CUDA_TRY(s.download(0, 0));
+    memcpy(out_host, s.h(0), 8);
     return SVT_B200_OK;
 }
 
@@ -295,59 +294,46 @@ int svt_b200_tf_planewise_block_host(int32_t bit_depth, int32_t chroma, const vo
         return SVT_B200_ERR_ARG;
     }
     const int es = bit_depth > 8 ? 2 : 1, uw = bw / 2, uh = bh / 2;
-    // packed staging: [src y | src u | src v | pre y | pre u | pre v] samples, then accum x3 (u32), count x3 (u16), block
+    // [src y | src u | src v | pre y | pre u | pre v] samples, then accum x3 (u32), count x3 (u16), block
     const size_t ny = (size_t)bw * bh, nc = (size_t)uw * uh;
-    auto al = [](size_t v) { return (v + 15) & ~(size_t)15; };
-    size_t off[14], o = 0;
-    const size_t sizes[13] = {ny * es, nc * es, nc * es, ny * es, nc * es, nc * es, ny * 4, nc * 4, nc * 4, ny * 2, nc * 2, nc * 2, sizeof(TfBlockDev)};
-    for (int i = 0; i < 13; i++) off[i] = o, o += al(sizes[i]);
-    off[13] = o;
-    ThreadCtx &c = tls();
-    c.reserve(o);
-    auto pack = [&](size_t dst, const void *src, int stride, int w, int h, int esz) {
-        for (int r = 0; r < h; r++) memcpy(c.h + dst + (size_t)r * w * esz, (const uint8_t *)src + (size_t)r * stride * esz, (size_t)w * esz);
-    };
-    pack(off[0], y_src, y_src_stride, bw, bh, es);
-    pack(off[3], y_pre, y_pre_stride, bw, bh, es);
-    pack(off[6], y_accum, y_pre_stride, bw, bh, 4);
-    pack(off[9], y_count, y_pre_stride, bw, bh, 2);
+    Staging s({ny * es, nc * es, nc * es, ny * es, nc * es, nc * es, ny * 4, nc * 4, nc * 4, ny * 2, nc * 2, nc * 2, sizeof(TfBlockDev)});
+    SVTB_CUDA_TRY(s.status());
+    s.put_rows(0, y_src, y_src_stride, es, bw, bh);
+    s.put_rows(3, y_pre, y_pre_stride, es, bw, bh);
+    s.put_rows(6, y_accum, y_pre_stride, 4, bw, bh);
+    s.put_rows(9, y_count, y_pre_stride, 2, bw, bh);
     if (chroma) {
-        pack(off[1], u_src, uv_src_stride, uw, uh, es);
-        pack(off[2], v_src, uv_src_stride, uw, uh, es);
-        pack(off[4], u_pre, uv_pre_stride, uw, uh, es);
-        pack(off[5], v_pre, uv_pre_stride, uw, uh, es);
-        pack(off[7], u_accum, uv_pre_stride, uw, uh, 4);
-        pack(off[8], v_accum, uv_pre_stride, uw, uh, 4);
-        pack(off[10], u_count, uv_pre_stride, uw, uh, 2);
-        pack(off[11], v_count, uv_pre_stride, uw, uh, 2);
+        s.put_rows(1, u_src, uv_src_stride, es, uw, uh);
+        s.put_rows(2, v_src, uv_src_stride, es, uw, uh);
+        s.put_rows(4, u_pre, uv_pre_stride, es, uw, uh);
+        s.put_rows(5, v_pre, uv_pre_stride, es, uw, uh);
+        s.put_rows(7, u_accum, uv_pre_stride, 4, uw, uh);
+        s.put_rows(8, v_accum, uv_pre_stride, 4, uw, uh);
+        s.put_rows(10, u_count, uv_pre_stride, 2, uw, uh);
+        s.put_rows(11, v_count, uv_pre_stride, 2, uw, uh);
     }
-    TfBlockDev blk;
-    blk.x = blk.y = 0;
-    for (int i = 0; i < 4; i++) blk.block_error[i] = block_error4[i], blk.d_factor[i] = d_factor4[i];
-    memcpy(c.h + off[12], &blk, sizeof(blk));
-    SVTB_CUDA_TRY(cudaMemcpyAsync(c.d, c.h, o, cudaMemcpyHostToDevice, c.stream));
-    SvtB200Frame fs = {c.d + off[0], c.d + off[1], c.d + off[2], (int32_t)bw, (int32_t)uw, (int32_t)bw, (int32_t)bh, bit_depth};
-    SvtB200Frame fp = {c.d + off[3], c.d + off[4], c.d + off[5], (int32_t)bw, (int32_t)uw, (int32_t)bw, (int32_t)bh, bit_depth};
+    TfBlockDev *blk = s.h<TfBlockDev>(12);
+    blk->x = blk->y = 0;
+    for (int i = 0; i < 4; i++) blk->block_error[i] = block_error4[i], blk->d_factor[i] = d_factor4[i];
+    SVTB_CUDA_TRY(s.upload(0, 12));
+    SvtB200Frame fs = {s.d(0), s.d(1), s.d(2), (int32_t)bw, (int32_t)uw, (int32_t)bw, (int32_t)bh, bit_depth};
+    SvtB200Frame fp = {s.d(3), s.d(4), s.d(5), (int32_t)bw, (int32_t)uw, (int32_t)bw, (int32_t)bh, bit_depth};
     SvtB200TfAccum acc;
-    for (int i = 0; i < 3; i++) acc.accum[i] = (uint32_t *)(c.d + off[6 + i]), acc.count[i] = (uint16_t *)(c.d + off[9 + i]);
+    for (int i = 0; i < 3; i++) acc.accum[i] = s.d<uint32_t>(6 + i), acc.count[i] = s.d<uint16_t>(9 + i);
     acc.stride_y = bw, acc.stride_c = uw;
     SvtB200TfParams p;
     for (int i = 0; i < 3; i++) p.den[i] = den3[i];
     p.chroma = chroma, p.block_w = bw, p.block_h = bh;
-    const int rc = svt_b200_tf_planewise(&p, &fs, &fp, (const SvtB200TfBlock *)(c.d + off[12]), 1, &acc, c.stream);
+    const int rc = svt_b200_tf_planewise(&p, &fs, &fp, s.d<const SvtB200TfBlock>(12), 1, &acc, s.stream());
     if (rc) return rc;
-    SVTB_CUDA_TRY(cudaMemcpyAsync(c.h + off[6], c.d + off[6], off[12] - off[6], cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_TRY(cudaStreamSynchronize(c.stream));
-    auto unpack = [&](void *dst, int stride, size_t src, int w, int h, int esz) {
-        for (int r = 0; r < h; r++) memcpy((uint8_t *)dst + (size_t)r * stride * esz, c.h + src + (size_t)r * w * esz, (size_t)w * esz);
-    };
-    unpack(y_accum, y_pre_stride, off[6], bw, bh, 4);
-    unpack(y_count, y_pre_stride, off[9], bw, bh, 2);
+    SVTB_CUDA_TRY(s.download(6, 11));
+    s.get_rows(6, y_accum, y_pre_stride, 4, bw, bh);
+    s.get_rows(9, y_count, y_pre_stride, 2, bw, bh);
     if (chroma) {
-        unpack(u_accum, uv_pre_stride, off[7], uw, uh, 4);
-        unpack(v_accum, uv_pre_stride, off[8], uw, uh, 4);
-        unpack(u_count, uv_pre_stride, off[10], uw, uh, 2);
-        unpack(v_count, uv_pre_stride, off[11], uw, uh, 2);
+        s.get_rows(7, u_accum, uv_pre_stride, 4, uw, uh);
+        s.get_rows(8, v_accum, uv_pre_stride, 4, uw, uh);
+        s.get_rows(10, u_count, uv_pre_stride, 2, uw, uh);
+        s.get_rows(11, v_count, uv_pre_stride, 2, uw, uh);
     }
     return SVT_B200_OK;
 }

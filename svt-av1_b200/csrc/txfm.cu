@@ -561,29 +561,26 @@ static void fwd_dropin(int16_t *input, int32_t *output, uint32_t stride, int tx_
     txfm_tables_init();
     tx_attrs();
     const int w = h_txw[tx_size], h = h_txh[tx_size];
-    ThreadCtx &c = tls();
-    const size_t in_bytes = (size_t)w * h * 2, out_off = (in_bytes + 15) & ~(size_t)15, e_off = out_off + (size_t)w * h * 4;
-    c.reserve(e_off + 16);
-    int16_t *hi = (int16_t *)c.h;
-    for (int r = 0; r < h; r++) memcpy(hi + (size_t)r * w, input + (size_t)r * stride, (size_t)w * 2);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, in_bytes, cudaMemcpyHostToDevice, c.stream));
+    Staging s({(size_t)w * h * 2, (size_t)w * h * 4, 8});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, input, stride, 2, w, h);
+    SVTB_CUDA_FATAL(s.upload(0, 0));
     FwdArgs a;
-    a.in = (const int16_t *)c.d;
+    a.in = s.d<const int16_t>(0);
     a.in_block_stride = 0;
     a.in_stride = w;
-    a.out = (int32_t *)(c.d + out_off);
+    a.out = s.d<int32_t>(1);
     a.tx_types = nullptr;
     a.tx_type = tx_type;
     a.tx_size = tx_size;
     a.n_blocks = 1;
     a.repack64 = repack;
     a.pf_shift = pf_shift;
-    a.energy = (uint64_t *)(c.d + e_off);
-    SVTB_LAUNCH(fwd_txfm_kernel, 1, TX_NT, tx_smem_bytes(tx_size), c.stream, a);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + out_off, c.d + out_off, (size_t)w * h * 4 + 16, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    memcpy(output, c.h + out_off, (size_t)w * h * 4);
-    if (energy_out) memcpy(energy_out, c.h + e_off, 8);
+    a.energy = s.d<uint64_t>(2);
+    SVTB_LAUNCH(fwd_txfm_kernel, 1, TX_NT, tx_smem_bytes(tx_size), s.stream(), a);
+    SVTB_CUDA_FATAL(s.download(1, 2));
+    memcpy(output, s.h(1), (size_t)w * h * 4);
+    if (energy_out) memcpy(energy_out, s.h(2), 8);
 }
 
 static void inv_dropin(const int32_t *input, uint16_t *output_r, int32_t stride_r, uint16_t *output_w, int32_t stride_w,
@@ -592,51 +589,47 @@ static void inv_dropin(const int32_t *input, uint16_t *output_r, int32_t stride_
     tx_attrs();
     const int w = h_txw[tx_size], h = h_txh[tx_size];
     const int iw = w > 32 ? 32 : w, ih = h > 32 ? 32 : h;
-    ThreadCtx &c = tls();
-    const size_t in_bytes = (size_t)iw * ih * 4, p_off = (in_bytes + 15) & ~(size_t)15, r_off = p_off + (size_t)w * h * 2;
-    c.reserve(r_off + (size_t)w * h * 2);
-    memcpy(c.h, input, in_bytes);
-    uint16_t *hp = (uint16_t *)(c.h + p_off);
-    for (int r = 0; r < h; r++) memcpy(hp + (size_t)r * w, output_r + (size_t)r * stride_r, (size_t)w * 2);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, r_off, cudaMemcpyHostToDevice, c.stream));
+    Staging s({(size_t)iw * ih * 4, (size_t)w * h * 2, (size_t)w * h * 2});
+    SVTB_CUDA_FATAL(s.status());
+    memcpy(s.h(0), input, (size_t)iw * ih * 4);
+    s.put_rows(1, output_r, stride_r, 2, w, h);
+    SVTB_CUDA_FATAL(s.upload(0, 1));
     InvArgs a;
-    a.in = (const int32_t *)c.d;
-    a.pred = (const uint16_t *)(c.d + p_off);
-    a.recon = (uint16_t *)(c.d + r_off);
+    a.in = s.d<const int32_t>(0);
+    a.pred = s.d<const uint16_t>(1);
+    a.recon = s.d<uint16_t>(2);
     a.pred_block_stride = a.recon_block_stride = 0;
     a.stride_r = a.stride_w = w;
     a.tx_type = tx_type;
     a.tx_size = tx_size;
     a.n_blocks = 1;
     a.bd = bd;
-    SVTB_LAUNCH(inv_txfm_kernel, 1, TX_NT, tx_smem_bytes(tx_size), c.stream, a);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + r_off, c.d + r_off, (size_t)w * h * 2, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    const uint16_t *ho = (const uint16_t *)(c.h + r_off);
-    for (int r = 0; r < h; r++) memcpy(output_w + (size_t)r * stride_w, ho + (size_t)r * w, (size_t)w * 2);
+    SVTB_LAUNCH(inv_txfm_kernel, 1, TX_NT, tx_smem_bytes(tx_size), s.stream(), a);
+    SVTB_CUDA_FATAL(s.download(2, 2));
+    s.get_rows(2, output_w, stride_w, 2, w, h);
 }
 
 static void quant_dropin(int mode, const int32_t *coeff, intptr_t n, const int16_t *zbin, const int16_t *round,
                          const int16_t *quant, const int16_t *quant_shift, int32_t *qcoeff, int32_t *dqcoeff,
                          const int16_t *dequant, uint16_t *eob, const int16_t *scan, const uint8_t *qm, const uint8_t *iqm,
                          int log_scale) {
-    ThreadCtx &c = tls();
-    const size_t cb = (size_t)n * 4, s_off = cb, qm_off = s_off + (size_t)n * 2, iqm_off = qm_off + n, q_off = (iqm_off + n + 15) & ~(size_t)15,
-                 dq_off = q_off + cb, e_off = dq_off + cb;
-    c.reserve(e_off + 16);
-    memcpy(c.h, coeff, cb);
-    memcpy(c.h + s_off, scan, (size_t)n * 2);
-    if (qm) memcpy(c.h + qm_off, qm, n);
-    if (iqm) memcpy(c.h + iqm_off, iqm, n);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, q_off, cudaMemcpyHostToDevice, c.stream));
+    // coeff | scan | qm | iqm in, qcoeff | dqcoeff | eob out
+    const size_t cb = (size_t)n * 4;
+    Staging s({cb, (size_t)n * 2, (size_t)n, (size_t)n, cb, cb, 2});
+    SVTB_CUDA_FATAL(s.status());
+    memcpy(s.h(0), coeff, cb);
+    memcpy(s.h(1), scan, (size_t)n * 2);
+    if (qm) memcpy(s.h(2), qm, n);
+    if (iqm) memcpy(s.h(3), iqm, n);
+    SVTB_CUDA_FATAL(s.upload(0, 3));
     QuantArgs a;
-    a.coeff = (const int32_t *)c.d;
-    a.scan = (const int16_t *)(c.d + s_off);
-    a.qm = qm ? c.d + qm_off : nullptr;
-    a.iqm = iqm ? c.d + iqm_off : nullptr;
-    a.qcoeff = (int32_t *)(c.d + q_off);
-    a.dqcoeff = (int32_t *)(c.d + dq_off);
-    a.eob = (uint16_t *)(c.d + e_off);
+    a.coeff = s.d<const int32_t>(0);
+    a.scan = s.d<const int16_t>(1);
+    a.qm = qm ? s.d(2) : nullptr;
+    a.iqm = iqm ? s.d(3) : nullptr;
+    a.qcoeff = s.d<int32_t>(4);
+    a.dqcoeff = s.d<int32_t>(5);
+    a.eob = s.d<uint16_t>(6);
     for (int i = 0; i < 2; i++) {
         a.q.zbin[i] = zbin ? zbin[i] : 0;
         a.q.round[i] = round[i];
@@ -647,12 +640,11 @@ static void quant_dropin(int mode, const int32_t *coeff, intptr_t n, const int16
     a.n = (int)n;
     a.log_scale = log_scale;
     a.mode = mode;
-    SVTB_LAUNCH(quant_kernel, 1, 256, 0, c.stream, a);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + q_off, c.d + q_off, 2 * cb + 16, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    memcpy(qcoeff, c.h + q_off, cb);
-    memcpy(dqcoeff, c.h + dq_off, cb);
-    memcpy(eob, c.h + e_off, 2);
+    SVTB_LAUNCH(quant_kernel, 1, 256, 0, s.stream(), a);
+    SVTB_CUDA_FATAL(s.download(4, 6));
+    memcpy(qcoeff, s.h(4), cb);
+    memcpy(dqcoeff, s.h(5), cb);
+    memcpy(eob, s.h(6), 2);
 }
 
 } // namespace
@@ -790,23 +782,20 @@ void svt_av1_highbd_quantize_fp_cuda(const int32_t *coeff_ptr, intptr_t n_coeffs
 
 static void residual_dropin(const void *src, uint32_t ss, const void *pred, uint32_t ps, int16_t *res, uint32_t rs, uint32_t w,
                             uint32_t h, int hbd) {
-    ThreadCtx &c = tls();
-    const size_t e = hbd ? 2 : 1, pb = (size_t)w * h * e, p_off = (pb + 15) & ~(size_t)15, r_off = 2 * p_off;
-    c.reserve(r_off + (size_t)w * h * 2);
-    for (uint32_t y = 0; y < h; y++) {
-        memcpy(c.h + (size_t)y * w * e, (const uint8_t *)src + (size_t)y * ss * e, w * e);
-        memcpy(c.h + p_off + (size_t)y * w * e, (const uint8_t *)pred + (size_t)y * ps * e, w * e);
-    }
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, r_off, cudaMemcpyHostToDevice, c.stream));
+    const size_t e = hbd ? 2 : 1, pb = (size_t)w * h * e;
+    Staging s({pb, pb, (size_t)w * h * 2});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, src, ss, e, w, h);
+    s.put_rows(1, pred, ps, e, w, h);
+    SVTB_CUDA_FATAL(s.upload(0, 1));
     if (hbd)
-        SVTB_LAUNCH(residual_kernel<uint16_t>, 4, 256, 0, c.stream, (const uint16_t *)c.d, (int)w, (const uint16_t *)(c.d + p_off),
-                    (int)w, (int16_t *)(c.d + r_off), (int)w, (int)w, (int)h);
+        SVTB_LAUNCH(residual_kernel<uint16_t>, 4, 256, 0, s.stream(), s.d<const uint16_t>(0), (int)w, s.d<const uint16_t>(1), (int)w,
+                    s.d<int16_t>(2), (int)w, (int)w, (int)h);
     else
-        SVTB_LAUNCH(residual_kernel<uint8_t>, 4, 256, 0, c.stream, (const uint8_t *)c.d, (int)w, (const uint8_t *)(c.d + p_off),
-                    (int)w, (int16_t *)(c.d + r_off), (int)w, (int)w, (int)h);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h + r_off, c.d + r_off, (size_t)w * h * 2, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    for (uint32_t y = 0; y < h; y++) memcpy(res + (size_t)y * rs, c.h + r_off + (size_t)y * w * 2, (size_t)w * 2);
+        SVTB_LAUNCH(residual_kernel<uint8_t>, 4, 256, 0, s.stream(), s.d<const uint8_t>(0), (int)w, s.d<const uint8_t>(1), (int)w,
+                    s.d<int16_t>(2), (int)w, (int)w, (int)h);
+    SVTB_CUDA_FATAL(s.download(2, 2));
+    s.get_rows(2, res, rs, 2, w, h);
 }
 void svt_residual_kernel8bit_cuda(uint8_t *input, uint32_t input_stride, uint8_t *pred, uint32_t pred_stride, int16_t *residual,
                                   uint32_t residual_stride, uint32_t area_width, uint32_t area_height) {
@@ -846,18 +835,15 @@ __global__ void handle64_kernel(int32_t *io, int w, int h, unsigned long long *e
 
 extern "C" uint64_t svt_b200_handle_transform64(int32_t *output, int tx_size) {
     const int w = h_txw[tx_size], h = h_txh[tx_size];
-    ThreadCtx &c = tls();
     const size_t nb = (size_t)w * h * 4;
-    c.reserve(nb + 16);
-    memcpy(c.h, output, nb);
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.d, c.h, nb, cudaMemcpyHostToDevice, c.stream));
-    SVTB_LAUNCH(handle64_kernel, 1, 256, nb, c.stream, (int32_t *)c.d, w, h, (unsigned long long *)(c.d + nb));
-    SVTB_CUDA_FATAL(cudaMemcpyAsync(c.h, c.d, nb + 8, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_FATAL(cudaStreamSynchronize(c.stream));
-    memcpy(output, c.h, nb);
-    uint64_t e;
-    memcpy(&e, c.h + nb, 8);
-    return e;
+    Staging s({nb, 8});
+    SVTB_CUDA_FATAL(s.status());
+    memcpy(s.h(0), output, nb);
+    SVTB_CUDA_FATAL(s.upload(0, 0));
+    SVTB_LAUNCH(handle64_kernel, 1, 256, nb, s.stream(), s.d<int32_t>(0), w, h, s.d<unsigned long long>(1));
+    SVTB_CUDA_FATAL(s.download(0, 1));
+    memcpy(output, s.h(0), nb);
+    return *s.h<uint64_t>(1);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1120,12 +1106,13 @@ int svt_b200_encode_tus_ex(const SvtB200EncodeParamsEx *p, const SvtB200Frame *s
     for (int i = 0; i < n_tus; i++) order[i] = i;
     auto key = [&](int i) { return ((uint32_t)tus[i].tx_size << 24) | ((uint32_t)tus[i].pf_shape << 16) | tus[i].qset; };
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return key(a) < key(b); });
-    // staging: TuDev[n] | qoff[n] | out_idx[n] in pinned memory of the calling thread, one upload
-    ThreadCtx &c = tls();
-    c.reserve((size_t)n_tus * per_tu + 256);
-    TuDev *h_tu = reinterpret_cast<TuDev *>(c.h);
-    long long *h_qoff = reinterpret_cast<long long *>(c.h + (((size_t)n_tus * sizeof(TuDev) + 15) & ~(size_t)15));
-    int32_t *h_idx = reinterpret_cast<int32_t *>(reinterpret_cast<uint8_t *>(h_qoff) + (size_t)n_tus * sizeof(long long));
+    // pinned staging of the calling thread: TuDev[n], then qoff[n] | out_idx[n] as one region, so that the upload
+    // (at most n * per_tu + 255 bytes) fits the caller's scratch
+    Staging s({(size_t)n_tus * sizeof(TuDev), (size_t)n_tus * (sizeof(long long) + sizeof(int32_t))});
+    SVTB_CUDA_TRY(s.status());
+    TuDev *h_tu = s.h<TuDev>(0);
+    long long *h_qoff = s.h<long long>(1);
+    int32_t *h_idx = reinterpret_cast<int32_t *>(h_qoff + n_tus);
     for (int k = 0; k < n_tus; k++) {
         const SvtB200TuEx &t = tus[order[k]];
         h_tu[k] = TuDev{t.x, t.y, t.plane, t.tx_type};
@@ -1133,12 +1120,11 @@ int svt_b200_encode_tus_ex(const SvtB200EncodeParamsEx *p, const SvtB200Frame *s
         h_idx[k] = order[k];
     }
     uint8_t *dsc = reinterpret_cast<uint8_t *>(scratch);
-    const size_t total = (size_t)(reinterpret_cast<uint8_t *>(h_idx + n_tus) - c.h);
     cudaStream_t st = (cudaStream_t)stream;
-    SVTB_CUDA_TRY(cudaMemcpyAsync(dsc, c.h, total, cudaMemcpyHostToDevice, st));
+    SVTB_CUDA_TRY(cudaMemcpyAsync(dsc, h_tu, s.span(0, 1), cudaMemcpyHostToDevice, st));
     const TuDev *d_tu = reinterpret_cast<const TuDev *>(dsc);
-    const long long *d_qoff = reinterpret_cast<const long long *>(dsc + (reinterpret_cast<uint8_t *>(h_qoff) - c.h));
-    const int32_t *d_idx = reinterpret_cast<const int32_t *>(dsc + (reinterpret_cast<uint8_t *>(h_idx) - c.h));
+    const long long *d_qoff = reinterpret_cast<const long long *>(dsc + s.off(1));
+    const int32_t *d_idx = reinterpret_cast<const int32_t *>(d_qoff + n_tus);
     int rc = SVT_B200_OK;
     for (int k0 = 0; k0 < n_tus && rc == SVT_B200_OK;) {
         int k1 = k0;
@@ -1248,17 +1234,15 @@ int svt_b200_ois_dc_picture_host(const uint8_t *y, int32_t stride, int32_t width
         return SVT_B200_ERR_ARG;
     }
     const int n_mb = ((width + 15) / 16) * ((height + 15) / 16);
-    const size_t o_cost = ((size_t)width * height + 255) & ~(size_t)255, total = o_cost + (size_t)n_mb * 8;
-    ThreadCtx &c = tls();
-    c.reserve(total);
-    for (int r = 0; r < height; r++) memcpy(c.h + (size_t)r * width, y + (size_t)r * stride, width);
-    SVTB_CUDA_TRY(cudaMemcpyAsync(c.d, c.h, (size_t)width * height, cudaMemcpyHostToDevice, c.stream));
-    SvtB200Frame f = {c.d, nullptr, nullptr, width, 0, width, height, 8};
-    const int rc = svt_b200_ois_dc_picture(&f, (int64_t *)(c.d + o_cost), c.stream);
+    Staging s({(size_t)width * height, (size_t)n_mb * 8});
+    SVTB_CUDA_TRY(s.status());
+    s.put_rows(0, y, stride, 1, width, height);
+    SVTB_CUDA_TRY(s.upload(0, 0));
+    SvtB200Frame f = {s.d(0), nullptr, nullptr, width, 0, width, height, 8};
+    const int rc = svt_b200_ois_dc_picture(&f, s.d<int64_t>(1), s.stream());
     if (rc) return rc;
-    SVTB_CUDA_TRY(cudaMemcpyAsync(c.h + o_cost, c.d + o_cost, (size_t)n_mb * 8, cudaMemcpyDeviceToHost, c.stream));
-    SVTB_CUDA_TRY(cudaStreamSynchronize(c.stream));
-    memcpy(cost, c.h + o_cost, (size_t)n_mb * 8);
+    SVTB_CUDA_TRY(s.download(1, 1));
+    memcpy(cost, s.h(1), (size_t)n_mb * 8);
     return SVT_B200_OK;
 }
 }
