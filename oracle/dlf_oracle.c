@@ -196,10 +196,12 @@ void orc_frame_sse(const SvtB200Frame *a, const SvtB200Frame *b, uint64_t *sse) 
 
 /* ---- svt_av1_loop_filter_frame_init (Common/Codec/EbDeblockingCommon.c:78-145) as a table over the level class
  *      cls = segment_id * 16 + ref_frame[0] * 2 + mode_lf_lut[mode] -------------------------------------------- */
-void orc_lf_level_lut(const SvtB200LfFrameInit *init, const int32_t levels[4], uint8_t lut[3][2][128]) {
+/* plane_start as frame_init's: a call that starts at a chroma plane fills that plane's table even when both luma levels
+ * are 0 (the level search's chroma trials, svt_av1_loop_filter_frame(plane, plane + 1)). */
+static void level_lut(const SvtB200LfFrameInit *init, const int32_t levels[4], int plane_start, uint8_t lut[3][2][128]) {
     static const int feature[3][2] = {{1, 2}, {3, 3}, {4, 4}}; /* seg_lvl_lf_lut */
     memset(lut, 0, 3 * 2 * 128);
-    for (int plane = 0; plane < 3; plane++) {
+    for (int plane = plane_start; plane < 3; plane++) {
         const int lv[2] = {plane == 0 ? levels[0] : levels[1 + plane], plane == 0 ? levels[1] : levels[1 + plane]};
         if (plane == 0 && !lv[0] && !lv[1]) break;
         if (plane && !lv[0]) continue;
@@ -220,6 +222,9 @@ void orc_lf_level_lut(const SvtB200LfFrameInit *init, const int32_t levels[4], u
             }
         }
     }
+}
+void orc_lf_level_lut(const SvtB200LfFrameInit *init, const int32_t levels[4], uint8_t lut[3][2][128]) {
+    level_lut(init, levels, 0, lut);
 }
 
 /* ---- svt_av1_pick_filter_level (Encoder/Codec/EbDeblockingFilter.c:1193-1297) -------------------------------- */
@@ -247,7 +252,7 @@ static int64_t try_level(PickState *st, int level, int plane, int dir) { /* try_
         st->hdr[1 + plane] = level;
     }
     uint8_t lut[3][2][128];
-    orc_lf_level_lut(&st->p->init, st->hdr, lut);
+    level_lut(&st->p->init, st->hdr, plane, lut);
     const SvtB200DlfParams *g = &st->p->dlf;
     for (int r = 0; r < g->mi_rows; r++)
         for (int c = 0; c < g->mi_cols; c++) {

@@ -470,13 +470,14 @@ int svt_b200_dlf_frame_lut(const SvtB200DlfParams *p, const SvtB200Frame *frame,
     return dlf_frame_impl(p, frame, mi, lut, stream);
 }
 
-// svt_av1_loop_filter_frame_init (EbDeblockingCommon.c:78-145): lvl[plane][seg][dir][ref][mode] as lut[plane][dir][class]
-int svt_b200_lf_level_lut(const SvtB200LfFrameInit *init, const int32_t levels[4], uint8_t lut[3][2][128]) {
-    if (!init || !levels || !lut) return SVT_B200_ERR_ARG;
+// svt_av1_loop_filter_frame_init (EbDeblockingCommon.c:78-145): lvl[plane][seg][dir][ref][mode] as lut[plane][dir][class].
+// The planes from plane_start on, as frame_init's loop: a table started at a chroma plane is filled even when both luma
+// levels are 0 (the chroma trials of the level search filter plane..plane+1 only).
+static void lf_level_lut(const SvtB200LfFrameInit *init, const int32_t levels[4], int plane_start, uint8_t lut[3][2][128]) {
     static const int seg_lvl_lf_lut[3][2] = {{1, 2}, {3, 3}, {4, 4}}; // SEG_LVL_ALT_LF_Y_V, _Y_H, _U, _V
     const int filt[3] = {levels[0], levels[2], levels[3]}, filt_r[3] = {levels[1], levels[2], levels[3]};
     memset(lut, 0, 3 * 2 * 128);
-    for (int plane = 0; plane < 3; plane++) {
+    for (int plane = plane_start; plane < 3; plane++) {
         if (plane == 0 && !filt[0] && !filt_r[0]) break;
         if (plane && !filt[plane]) continue;
         for (int seg = 0; seg < 8; seg++)
@@ -501,6 +502,10 @@ int svt_b200_lf_level_lut(const SvtB200LfFrameInit *init, const int32_t levels[4
                     }
             }
     }
+}
+int svt_b200_lf_level_lut(const SvtB200LfFrameInit *init, const int32_t levels[4], uint8_t lut[3][2][128]) {
+    if (!init || !levels || !lut) return SVT_B200_ERR_ARG;
+    lf_level_lut(init, levels, 0, lut);
     return SVT_B200_OK;
 }
 
@@ -536,7 +541,7 @@ int64_t try_filter(PickCtx &c, int level, int plane, int dir) {
     // the trial levels stay in the frame header (set base filters ... :1007-1014)
     for (int i = 0; i < 4; i++) c.cur[i] = lv[i];
     uint8_t(*lut)[2][128] = reinterpret_cast<uint8_t(*)[2][128]>(c.h_lut);
-    svt_b200_lf_level_lut(&c.p->init, lv, lut);
+    lf_level_lut(&c.p->init, lv, plane, lut);
     SvtB200DlfParams dp = c.p->dlf;
     dp.sharpness = 0;
     dp.filter_level[0] = lv[0], dp.filter_level[1] = lv[1], dp.filter_level_u = lv[2], dp.filter_level_v = lv[3];
