@@ -7,17 +7,21 @@
 //   svt_ext_sad_calculation_8x8_16x16_c / _32x32_64x64_c  :122-225
 //   motion_estimate_sb and everything below it (:852-3041) for a whole picture.
 //
-// Design (B200-first, not a port of the AVX2 mpsadbw code):
-//   * one CTA per (super-block, reference picture); the 64x64 source block and the reference search
-//     window are staged once into shared memory and every candidate position is evaluated from there,
-//     so HBM traffic is the algorithmic minimum (source + window once per SB-ref);
-//   * SAD arithmetic uses the native VABSDIFF4.U8.ACC (4 abs-diffs + accumulate per lane-op); a thread
-//     owns FOUR horizontally adjacent search positions so three aligned LDS words serve all four through
-//     funnel shifts (SHF) — 4.5 issue slots per 8-pixel row-position instead of 9;
+// Design (not a port of the AVX2 mpsadbw code):
+//   * one picture is two launches and no host sync, each with one CTA per (super-block, reference picture):
+//     - the three HME levels (one body, hme_sb), in one of two regimes chosen per picture by me_launch_plan.
+//       hme_kernel_staged: every search region's window of a level and the source block are in shared memory at once
+//       and the regions are searched concurrently.  hme_kernel_chunked, when a level's staged need exceeds HME_FAST_SMEM
+//       (presets 0-1 at reference distances above one, or with the 4K-class table): block_search runs the
+//       regions one after another, each window chunked through HME_SMEM_BYTES;
+//     - fullpel_kernel<SUB>, the integer full-pel search; the SB's last CTA also runs the SB epilogue;
+//   * SAD arithmetic uses the native VABSDIFF4.U8.ACC (4 abs-diffs + accumulate per lane-op); a task is Q
+//     search positions of one row with the same byte alignment, so one funnel-shifted (SHF) copy of a window
+//     row feeds all Q positions (DESIGN.md §4);
 //   * "first minimum in raster order" (the reference's strict `<` running best) is an argmin over the key
 //     (sad << 32 | raster_index): REDUX.MIN warp reductions + one shared-memory atomicMin per warp;
 //   * the data-dependent glue between the stages (search-centre choice, reference pruning, search-region
-//     shrinking, candidate list) runs on-device too, so one picture is three launches and no host sync.
+//     shrinking, candidate list) runs on-device, in the CTA that completes an SB in each kernel.
 #include "common.cuh"
 
 using namespace svtb200;
@@ -37,12 +41,64 @@ __constant__ uint8_t c_tab8[64] = {0,  1,  4,  5,  16, 17, 20, 21, 2,  3,  6,  7
 // The reference's search-window clamp, statement for statement (e.g. EbMotionEstimation.c:927-975): the
 // left/top clamp moves the origin and then re-tests the corrected origin (never true), so only the
 // right/bottom clamp shrinks the size.
-__device__ __forceinline__ void clamp_window(int origin, int pad, int pic_size, int &ao, int &size) {
+__host__ __device__ __forceinline__ void clamp_window(int origin, int pad, int pic_size, int &ao, int &size) {
     if (origin + ao < -pad) ao = -pad - origin;
     if (origin + ao > pic_size - 1) ao = ao - ((origin + ao) - (pic_size - 1));
     if (origin + ao + size > pic_size) size = max(1, size - ((origin + ao + size) - pic_size));
 }
-__device__ __forceinline__ int scaled_dist(int dist) { return ((dist * 5) / 8) + ((dist % 8) == 0 ? 0 : 1); }
+__host__ __device__ __forceinline__ int scaled_dist(int dist) { return ((dist * 5) / 8) + ((dist % 8) == 0 ? 0 : 1); }
+
+// The search window of HME region (rx, ry) at `level` (0: 1/16, 1: 1/4, 2: full resolution), hme_level_0/1/2
+// (:852-1318): offset (xo, yo) from the block and size, at the level's resolution.  Level 0 is centred on the block and
+// scaled by the reference's distance multiplier `mult` (scaled_dist * 100); levels 1 and 2 are centred on the previous
+// level's result (cx, cy), like (ox, oy) the block origin, in full-resolution samples.
+struct HmeWindow {
+    int xo, yo, saw, sah;
+};
+__host__ __device__ __forceinline__ HmeWindow hme_window(const SvtB200MeParams &p, int level, int rx, int ry, int mult, int cx, int cy,
+                                                         int ox, int oy) {
+    const SvtB200Plane &pl = level == 0 ? p.sixteenth : level == 1 ? p.quarter : p.full;
+    const int shf = 2 - level, o_x = ox >> shf, o_y = oy >> shf;
+    HmeWindow w;
+    if (level == 0) {
+        w.saw = min((int)(int16_t)((((p.hme_level0_search_area_in_width_array[rx] * mult) / 100) + 15) & ~0x0F),
+                    (int)(int16_t)((p.hme_level0_max_search_area_in_width_array[rx] + 15) & ~0x0F));
+        w.sah = min((int)(int16_t)((p.hme_level0_search_area_in_height_array[ry] * mult) / 100),
+                    (int)(int16_t)p.hme_level0_max_search_area_in_height_array[ry]);
+        int xdist = 0, ydist = 0;
+        for (int i = 0; i < rx; i++)
+            xdist += min((int)(int16_t)((p.hme_level0_search_area_in_width_array[i] * mult) / 100),
+                         (int)(int16_t)p.hme_level0_max_search_area_in_width_array[i]);
+        for (int i = 0; i < ry; i++)
+            ydist += min((int)(int16_t)((p.hme_level0_search_area_in_height_array[i] * mult) / 100),
+                         (int)(int16_t)p.hme_level0_max_search_area_in_height_array[i]);
+        w.xo = -(int)(int16_t)(min((p.hme_level0_total_search_area_width * mult) / 100, p.hme_level0_max_total_search_area_width) >> 1) +
+               xdist;
+        w.yo = -(int)(int16_t)(min((p.hme_level0_total_search_area_height * mult) / 100, p.hme_level0_max_total_search_area_height) >> 1) +
+               ydist;
+        clamp_window(o_x, pl.origin_x - 1, pl.width, w.xo, w.saw);
+        w.saw = w.saw < 16 ? w.saw : w.saw & ~0x0F;
+        clamp_window(o_y, pl.origin_y - 1, pl.height, w.yo, w.sah);
+    } else {
+        const int aw = level == 1 ? p.hme_level1_search_area_in_width_array[rx] : p.hme_level2_search_area_in_width_array[rx];
+        const int ah = level == 1 ? p.hme_level1_search_area_in_height_array[ry] : p.hme_level2_search_area_in_height_array[ry];
+        w.saw = (int16_t)((aw + 7) & ~0x07);
+        w.sah = ah;
+        w.xo = -(w.saw >> 1) + (cx >> shf);
+        w.yo = -(w.sah >> 1) + (cy >> shf);
+        clamp_window(o_x, level == 1 ? pl.origin_x - 1 : 63, pl.width, w.xo, w.saw);
+        w.saw = w.saw < 8 ? w.saw : w.saw & ~0x07;
+        clamp_window(o_y, level == 1 ? pl.origin_y - 1 : 63, pl.height, w.yo, w.sah);
+    }
+    return w;
+}
+
+// integer_search_sb's search area of a reference at scaled distance `dist`, before HME's search-area divisor, and the
+// window width it becomes (rounded up to a multiple of 8) once divided
+__host__ __device__ __forceinline__ int2 fp_search_area(const SvtB200MeParams &p, int dist) {
+    return make_int2(min(p.search_area_width * dist, p.max_me_search_width), min(p.search_area_height * dist, p.max_me_search_height));
+}
+__host__ __device__ __forceinline__ int fp_window_width(int w) { return (w + 7) & ~0x07; }
 
 // Stage `rows` rows of `nbytes` bytes (arbitrary alignment, global) into shared-memory words of pitch `wpw`:
 // one warp per row, one lane per 32-bit word, aligned LDG + funnel shift instead of byte loads.  Only the aligned
@@ -60,11 +116,6 @@ __device__ __forceinline__ void stage_rows_n(uint32_t *dst, int wpw, const uint8
             dst[row * wpw + wd] = __funnelshift_r(lo, hi, sh);
         }
     }
-}
-template <int NT>
-__device__ __forceinline__ void stage_rows(uint32_t *dst, int wpw, const uint8_t *__restrict__ src, ptrdiff_t stride, int rows,
-                                           int nbytes) {
-    stage_rows_n(dst, wpw, src, stride, rows, nbytes, NT / 32);
 }
 
 // -----------------------------------------------------------------------------------------------------
@@ -223,7 +274,7 @@ __device__ void derive_hme_state(const SvtB200MeParams &p, const RawHme *raw /*[
     }
 }
 
-// Tail of both HME kernels (thread 0): publish this (SB, reference) result; the CTA that completes the SB derives the
+// Tail of the HME kernel (thread 0): publish this (SB, reference) result; the CTA that completes the SB derives the
 // cross-reference state ONCE for the full-pel and finalize kernels (it was a serial prologue in each of their CTAs).
 __device__ void hme_publish(const MeDev &d, int sb, RawHme *out, const RawHme &w) {
     *out = w;
@@ -243,155 +294,15 @@ __device__ void hme_publish(const MeDev &d, int sb, RawHme *out, const RawHme &w
     }
 }
 
-constexpr int HME_SMEM_BYTES = 40 * 1024;
-
-// Kernel A (generic fallback, any window size: regions searched one after another, windows chunked through
-// shared memory): hierarchical ME, one CTA per (SB, reference). hme_level_0/1/2 (:852-1318) for the 2x2 search
-// regions, then the region choice of set_final_seach_centre_sb.
-__global__ void __launch_bounds__(NT_SEARCH) hme_kernel_generic(const __grid_constant__ MeDev d) {
-    extern __shared__ uint32_t smem[];
-    __shared__ uint64_t s_red[NT_SEARCH / 32];
-    const SvtB200MeParams &p = d.p;
-    const int sb = blockIdx.x, slot = blockIdx.y;
-    const int l = d.slot_l[slot], r = d.slot_r[slot];
-    RawHme *out = d.raw + (size_t)sb * 8 + l * 4 + r;
-    const bool active = (p.temporal_layer_index > 0 || l == 0) && p.enable_hme_flag &&
-                        (p.enable_hme_level0_flag || p.enable_hme_level1_flag || p.enable_hme_level2_flag);
-    if (!active) {
-        if (threadIdx.x == 0) {
-            RawHme z = {0, 0, 0, 0};
-            hme_publish(d, sb, out, z);
-        }
-        return;
-    }
-    const int sx = sb % d.sbs_x, sy = sb / d.sbs_x;
-    const int ox = sx * 64, oy = sy * 64;
-    const int sbw = min(p.full.width - ox, 64), sbh = min(p.full.height - oy, 64);
-    const int sub = p.hme_search_method != 0;
-    const int mult = scaled_dist(p.ref_dist[l][r]) * 100;
-    const int nrw = p.number_hme_search_region_in_width, nrh = p.number_hme_search_region_in_height;
-    const SvtB200MePlanes &rp = d.refs[l][r];
-
-    uint64_t best_sad = 0;
-    int best_x = 0, best_y = 0;
-    bool first = true;
-    for (int ry = 0; ry < nrh; ry++)
-        for (int rx = 0; rx < nrw; rx++) {
-            int cx = 0, cy = 0;
-            uint64_t csad = 0;
-            if (p.enable_hme_level0_flag) { // hme_level_0, 1/16 resolution
-                const SvtB200Plane &pl = p.sixteenth;
-                const int o_x = ox >> 2, o_y = oy >> 2, bw = sbw >> 2, bh = sbh >> 2;
-                int saw = min((int)(int16_t)((((p.hme_level0_search_area_in_width_array[rx] * mult) / 100) + 15) & ~0x0F),
-                              (int)(int16_t)((p.hme_level0_max_search_area_in_width_array[rx] + 15) & ~0x0F));
-                int sah = min((int)(int16_t)((p.hme_level0_search_area_in_height_array[ry] * mult) / 100),
-                              (int)(int16_t)p.hme_level0_max_search_area_in_height_array[ry]);
-                int xdist = 0, ydist = 0;
-                for (int i = 0; i < rx; i++)
-                    xdist += min((int)(int16_t)((p.hme_level0_search_area_in_width_array[i] * mult) / 100),
-                                 (int)(int16_t)p.hme_level0_max_search_area_in_width_array[i]);
-                for (int i = 0; i < ry; i++)
-                    ydist += min((int)(int16_t)((p.hme_level0_search_area_in_height_array[i] * mult) / 100),
-                                 (int)(int16_t)p.hme_level0_max_search_area_in_height_array[i]);
-                int xo = -(int)(int16_t)(min((p.hme_level0_total_search_area_width * mult) / 100,
-                                             p.hme_level0_max_total_search_area_width) >> 1) + xdist;
-                int yo = -(int)(int16_t)(min((p.hme_level0_total_search_area_height * mult) / 100,
-                                             p.hme_level0_max_total_search_area_height) >> 1) + ydist;
-                clamp_window(o_x, pl.origin_x - 1, pl.width, xo, saw);
-                saw = saw < 16 ? saw : saw & ~0x0F;
-                clamp_window(o_y, pl.origin_y - 1, pl.height, yo, sah);
-                const uint8_t *s = d.src.sixteenth + (size_t)(pl.origin_y + o_y) * pl.stride + pl.origin_x + o_x;
-                const uint8_t *f = rp.sixteenth + (size_t)(pl.origin_y + o_y + yo) * pl.stride + pl.origin_x + o_x + xo;
-                uint64_t key = block_search<NT_SEARCH>(s, sub ? pl.stride * 2 : pl.stride, f, pl.stride, sub ? 2 : 1, bw,
-                                                       sub ? bh >> 1 : bh, saw, sah, smem, HME_SMEM_BYTES, s_red);
-                uint32_t sad = (uint32_t)(key >> 32), idx = (uint32_t)key;
-                int kx = 0, ky = 0;
-                uint64_t lsad = 0xffffff; // svt_sad_loop_kernel_c start value; centre untouched if never beaten
-                if (sad < 0xffffffu) {
-                    lsad = sad;
-                    kx = idx % saw;
-                    ky = idx / saw;
-                }
-                csad = sub ? lsad * 2 : lsad;
-                cx = (int16_t)((kx + xo) * 4);
-                cy = (int16_t)((ky + yo) * 4);
-            }
-            if (p.enable_hme_level1_flag) { // hme_level_1, 1/4 resolution
-                const SvtB200Plane &pl = p.quarter;
-                const int o_x = ox >> 1, o_y = oy >> 1, bw = sbw >> 1, bh = sbh >> 1;
-                int saw = (int16_t)((p.hme_level1_search_area_in_width_array[rx] + 7) & ~0x07);
-                int sah = p.hme_level1_search_area_in_height_array[ry];
-                int xo = -(saw >> 1) + (cx >> 1), yo = -(sah >> 1) + (cy >> 1);
-                clamp_window(o_x, pl.origin_x - 1, pl.width, xo, saw);
-                saw = saw < 8 ? saw : saw & ~0x07;
-                clamp_window(o_y, pl.origin_y - 1, pl.height, yo, sah);
-                const uint8_t *s = d.src.quarter + (size_t)(pl.origin_y + o_y) * pl.stride + pl.origin_x + o_x;
-                const uint8_t *f = rp.quarter + (size_t)(pl.origin_y + o_y + yo) * pl.stride + pl.origin_x + o_x + xo;
-                uint64_t key = block_search<NT_SEARCH>(s, sub ? pl.stride * 2 : pl.stride, f, pl.stride, sub ? 2 : 1, bw,
-                                                       sub ? bh >> 1 : bh, saw, sah, smem, HME_SMEM_BYTES, s_red);
-                uint32_t sad = (uint32_t)(key >> 32), idx = (uint32_t)key;
-                int kx = 0, ky = 0;
-                uint64_t lsad = 0xffffff;
-                if (sad < 0xffffffu) {
-                    lsad = sad;
-                    kx = idx % saw;
-                    ky = idx / saw;
-                }
-                csad = sub ? lsad * 2 : lsad;
-                cx = (int16_t)((kx + xo) * 2);
-                cy = (int16_t)((ky + yo) * 2);
-            }
-            if (p.enable_hme_level2_flag) { // hme_level_2, full resolution
-                const SvtB200Plane &pl = p.full;
-                int saw = (int16_t)((p.hme_level2_search_area_in_width_array[rx] + 7) & ~0x07);
-                int sah = p.hme_level2_search_area_in_height_array[ry];
-                int xo = -(saw >> 1) + cx, yo = -(sah >> 1) + cy;
-                clamp_window(ox, 63, pl.width, xo, saw);
-                saw = saw < 8 ? saw : saw & ~0x07;
-                clamp_window(oy, 63, pl.height, yo, sah);
-                const uint8_t *s = d.src.full + (size_t)(pl.origin_y + oy) * pl.stride + pl.origin_x + ox;
-                const uint8_t *f = rp.full + (size_t)(pl.origin_y + oy + yo) * pl.stride + pl.origin_x + ox + xo;
-                uint64_t key = block_search<NT_SEARCH>(s, sub ? pl.stride * 2 : pl.stride, f, pl.stride, sub ? 2 : 1, sbw,
-                                                       sub ? sbh >> 1 : sbh, saw, sah, smem, HME_SMEM_BYTES, s_red);
-                uint32_t sad = (uint32_t)(key >> 32), idx = (uint32_t)key;
-                int kx = 0, ky = 0;
-                uint64_t lsad = 0xffffff;
-                if (sad < 0xffffffu) {
-                    lsad = sad;
-                    kx = idx % saw;
-                    ky = idx / saw;
-                }
-                csad = sub ? lsad * 2 : lsad;
-                cx = (int16_t)(kx + xo);
-                cy = (int16_t)(ky + yo);
-            }
-            // set_final_seach_centre_sb: start from region (0,0), strict `<` over (ry outer, rx inner)
-            if (first || csad < best_sad) {
-                best_sad = csad;
-                best_x = cx;
-                best_y = cy;
-                first = false;
-            }
-        }
-    if (threadIdx.x == 0) {
-        RawHme w;
-        w.x = (int16_t)best_x;
-        w.y = (int16_t)best_y;
-        w.valid = 1;
-        w.sad = best_sad;
-        hme_publish(d, sb, out, w);
-    }
-}
-
-
-// ---- Kernel A (fast path): all 2x2 search regions of an HME level are searched concurrently ----------------
+// ---- HME, staged regime: all (up to 2x2) search regions of a level are searched concurrently ------------------
 // Per level: every region's window + the (shared) source block are staged once.  Full-width blocks (sbw == 64) use
 // the aligned-task scheme of the full-pel kernel: a task is Q positions of one search row with the same byte
 // alignment, x = 4Q*m + c + 4k, so that one shifted copy of the window row (W + Q - 1 SHF) feeds W*Q VABSDIFF4 and
 // all loads are 8/16-byte LDS.  The rows of a task are split over `tpp` threads so that the tiny level-1/2 areas
 // (8x3) still fill the CTA; every warp works for ONE region, so the per-region argmin is a warp reduction plus one
 // shared 64-bit atomicMin.  Ragged blocks (picture width not a multiple of 64) take hme_level_search below.
-constexpr int HME_FAST_SMEM = 64 * 1024;
+constexpr int HME_FAST_SMEM = 64 * 1024; // the most dynamic shared memory the staged regime is launched with
+constexpr int HME_SMEM_BYTES = 40 * 1024; // the chunked regime's block_search budget
 struct HmeJob {
     const uint8_t *ref; // search position (0,0)
     int xo, yo, saw, sah;
@@ -602,11 +513,11 @@ __device__ void hme_level_search(const uint8_t *__restrict__ src, int src_stride
     const int spw = (bw + 3) >> 2;
     uint32_t *s_src = smem;
     const uint32_t tail_mask = (bw & 3) ? ((1u << (8 * (bw & 3))) - 1u) : 0xffffffffu;
-    stage_rows<NT>(s_src, spw, src, src_stride, bh, bw); // the source block, once for all jobs
+    stage_rows_n(s_src, spw, src, src_stride, bh, bw, NT / 32); // the source block, once for all jobs
     const int span = (bh - 1) * k + 1;
     for (int j = 0; j < njobs; j++) {
         const HmeJob jb = jobs[j];
-        stage_rows<NT>(smem + jb.woff, jb.wpw, jb.ref, raw_stride, jb.sah - 1 + span, jb.saw - 1 + bw);
+        stage_rows_n(smem + jb.woff, jb.wpw, jb.ref, raw_stride, jb.sah - 1 + span, jb.saw - 1 + bw, NT / 32);
     }
     __syncthreads();
     for (int j = 0; j < njobs; j++) {
@@ -654,7 +565,63 @@ __device__ void hme_level_search(const uint8_t *__restrict__ src, int src_stride
     __syncthreads();
 }
 
-__global__ void __launch_bounds__(NT_SEARCH, 6) hme_kernel(const __grid_constant__ MeDev d) {
+// Staged regime, lanes 0..3 (one per search region; `jl`: the region exists) after the region's window is in `jb`:
+// window pitch and offset (words) after the source block, task ranges padded to whole warps, rows-per-task split and
+// key packing.  Prefix sums / maxima over the four lanes by shuffles (no serial section, one barrier).
+__device__ __forceinline__ void hme_task_layout(HmeJob &jb, bool jl, int bw, int bh, int k, bool aligned, int &s_tpp, int &s_ntasks,
+                                                int &s_kshift) {
+    const int tid = threadIdx.x;
+    if (jl) {
+        jb.q = (jb.saw & 15) ? 2 : 4;
+        jb.gpr = (jb.saw + 4 * jb.q - 1) / (4 * jb.q);
+        jb.magic = (uint32_t)((0x100000000ull + 4 * jb.gpr - 1) / (4 * jb.gpr));
+        jb.wpw = aligned ? hme_pitch_words(jb.saw, bw >> 2, jb.q) : ((jb.saw - 1 + bw + 3) >> 2) + 1;
+    }
+    const unsigned m4 = 0xfu;
+    const int wsz = jl ? jb.wpw * (jb.sah - 1 + (bh - 1) * k + 1) : 0;
+    int inc = wsz, v = __shfl_up_sync(m4, inc, 1);
+    if (tid >= 1) inc += v;
+    v = __shfl_up_sync(m4, inc, 2);
+    if (tid >= 2) inc += v;
+    jb.woff = ((bw + 3) >> 2) * bh + inc - wsz;
+    const int T = jl ? jb.sah * 4 * jb.gpr : 0;
+    int tpp = 32, tot = 0;
+    for (;; tpp >>= 1) {
+        const int pad = 32 / tpp;
+        jb.nt = (T + pad - 1) & ~(pad - 1);
+        inc = jb.nt;
+        v = __shfl_up_sync(m4, inc, 1);
+        if (tid >= 1) inc += v;
+        v = __shfl_up_sync(m4, inc, 2);
+        if (tid >= 2) inc += v;
+        tot = __shfl_sync(m4, inc, 3);
+        jb.t0 = inc - jb.nt;
+        if (tpp == 1 || (tpp <= bh && tot * tpp <= NT_SEARCH)) break; // same decision in all four lanes
+    }
+    int maxp = jl ? jb.saw * jb.sah : 1;
+    maxp = max(maxp, __shfl_xor_sync(m4, maxp, 1));
+    maxp = max(maxp, __shfl_xor_sync(m4, maxp, 2));
+    if (tid == 0) {
+        s_tpp = tpp;
+        s_ntasks = tot;
+        // packed 32-bit keys when (largest SAD of the level, largest position index) fit together
+        const int ibits = 32 - __clz(maxp - 1 > 0 ? maxp - 1 : 1);
+        const int sbits = 32 - __clz(255 * bw * bh);
+        s_kshift = (ibits + sbits <= 31) ? ibits : 0;
+    }
+}
+
+// Kernel A: hierarchical ME, one CTA per (SB, reference).  hme_level_0/1/2 (:852-1318) for the search regions, then the
+// region choice of set_final_seach_centre_sb.  Per level, lanes 0..3 place one region's window each (hme_window), the
+// CTA searches every region, and lanes 0..3 turn each region's key into its centre.  Only the search differs between the
+// regimes (me_launch_plan picks one per picture):
+//   STAGED:  every region's window is in shared memory at once: hme_level_search_aligned<W>, or hme_level_search for
+//            ragged picture widths;
+//   chunked: block_search runs the regions one after another, each window chunked through HME_SMEM_BYTES.
+// One body, two kernels, because the regimes need different launch bounds: the chunked kernel gives no minimum of CTAs
+// per SM (with one, even of 1, its call took 9 % longer at 1920x1080 preset 1 on an H100 SXM at 700 W).
+template <bool STAGED>
+__device__ __forceinline__ void hme_sb(const MeDev &d) {
     extern __shared__ uint4 smem4[];
     uint32_t *smem = reinterpret_cast<uint32_t *>(smem4);
     __shared__ HmeJob s_jobs[4];
@@ -699,110 +666,51 @@ __global__ void __launch_bounds__(NT_SEARCH, 6) hme_kernel(const __grid_constant
         const uint8_t *srcp = level == 0 ? d.src.sixteenth : level == 1 ? d.src.quarter : d.src.full;
         const uint8_t *refp = level == 0 ? rp.sixteenth : level == 1 ? rp.quarter : rp.full;
         __syncthreads(); // previous level's results (s_cx/s_cy) are final; smem free
-        if (tid < 4) { // job geometry: the window arithmetic of hme_level_0/1/2, one lane per search region
+        if (tid < 4) { // one lane per search region, in (ry outer, rx inner) order
             const bool jl = tid < njobs;
             HmeJob jb;
             memset(&jb, 0, sizeof(jb));
             if (jl) {
-            const int rx = tid % nrw, ry = tid / nrw;
-            int saw, sah, xo, yo;
-            if (level == 0) {
-                saw = min((int)(int16_t)((((p.hme_level0_search_area_in_width_array[rx] * mult) / 100) + 15) & ~0x0F),
-                          (int)(int16_t)((p.hme_level0_max_search_area_in_width_array[rx] + 15) & ~0x0F));
-                sah = min((int)(int16_t)((p.hme_level0_search_area_in_height_array[ry] * mult) / 100),
-                          (int)(int16_t)p.hme_level0_max_search_area_in_height_array[ry]);
-                int xdist = 0, ydist = 0;
-                for (int i = 0; i < rx; i++)
-                    xdist += min((int)(int16_t)((p.hme_level0_search_area_in_width_array[i] * mult) / 100),
-                                 (int)(int16_t)p.hme_level0_max_search_area_in_width_array[i]);
-                for (int i = 0; i < ry; i++)
-                    ydist += min((int)(int16_t)((p.hme_level0_search_area_in_height_array[i] * mult) / 100),
-                                 (int)(int16_t)p.hme_level0_max_search_area_in_height_array[i]);
-                xo = -(int)(int16_t)(min((p.hme_level0_total_search_area_width * mult) / 100,
-                                         p.hme_level0_max_total_search_area_width) >> 1) + xdist;
-                yo = -(int)(int16_t)(min((p.hme_level0_total_search_area_height * mult) / 100,
-                                         p.hme_level0_max_total_search_area_height) >> 1) + ydist;
-                clamp_window(o_x, pl.origin_x - 1, pl.width, xo, saw);
-                saw = saw < 16 ? saw : saw & ~0x0F;
-                clamp_window(o_y, pl.origin_y - 1, pl.height, yo, sah);
-            } else {
-                const int aw = level == 1 ? p.hme_level1_search_area_in_width_array[rx] : p.hme_level2_search_area_in_width_array[rx];
-                const int ah = level == 1 ? p.hme_level1_search_area_in_height_array[ry] : p.hme_level2_search_area_in_height_array[ry];
-                saw = (int16_t)((aw + 7) & ~0x07);
-                sah = ah;
-                const int cx = level == 1 ? (s_cx[tid] >> 1) : s_cx[tid], cy = level == 1 ? (s_cy[tid] >> 1) : s_cy[tid];
-                xo = -(saw >> 1) + cx;
-                yo = -(sah >> 1) + cy;
-                clamp_window(o_x, level == 1 ? pl.origin_x - 1 : 63, pl.width, xo, saw);
-                saw = saw < 8 ? saw : saw & ~0x07;
-                clamp_window(o_y, level == 1 ? pl.origin_y - 1 : 63, pl.height, yo, sah);
+                const HmeWindow w = hme_window(p, level, tid % nrw, tid / nrw, mult, s_cx[tid], s_cy[tid], ox, oy);
+                jb.ref = refp + (size_t)(pl.origin_y + o_y + w.yo) * pl.stride + pl.origin_x + o_x + w.xo;
+                jb.xo = w.xo;
+                jb.yo = w.yo;
+                jb.saw = w.saw;
+                jb.sah = w.sah;
             }
-            jb.ref = refp + (size_t)(pl.origin_y + o_y + yo) * pl.stride + pl.origin_x + o_x + xo;
-            jb.xo = xo;
-            jb.yo = yo;
-            jb.saw = saw;
-            jb.sah = sah;
-            jb.q = (saw & 15) ? 2 : 4;
-            jb.gpr = (saw + 4 * jb.q - 1) / (4 * jb.q);
-            jb.magic = (uint32_t)((0x100000000ull + 4 * jb.gpr - 1) / (4 * jb.gpr));
-            jb.wpw = aligned ? hme_pitch_words(saw, bw >> 2, jb.q) : ((saw - 1 + bw + 3) >> 2) + 1;
-            }
-            // window offsets (words) after the source block, task ranges padded to whole warps, rows-per-task split and
-            // key packing: prefix sums / maxima over the four job lanes by shuffles (no serial section, one barrier)
-            const unsigned m4 = 0xfu;
-            const int wsz = jl ? jb.wpw * (jb.sah - 1 + (bh - 1) * k + 1) : 0;
-            int inc = wsz, v = __shfl_up_sync(m4, inc, 1);
-            if (tid >= 1) inc += v;
-            v = __shfl_up_sync(m4, inc, 2);
-            if (tid >= 2) inc += v;
-            jb.woff = ((bw + 3) >> 2) * bh + inc - wsz;
-            const int T = jl ? jb.sah * 4 * jb.gpr : 0;
-            int tpp = 32, tot = 0;
-            for (;; tpp >>= 1) {
-                const int pad = 32 / tpp;
-                jb.nt = (T + pad - 1) & ~(pad - 1);
-                inc = jb.nt;
-                v = __shfl_up_sync(m4, inc, 1);
-                if (tid >= 1) inc += v;
-                v = __shfl_up_sync(m4, inc, 2);
-                if (tid >= 2) inc += v;
-                tot = __shfl_sync(m4, inc, 3);
-                jb.t0 = inc - jb.nt;
-                if (tpp == 1 || (tpp <= bh && tot * tpp <= NT_SEARCH)) break; // same decision in all four lanes
-            }
-            int maxp = jl ? jb.saw * jb.sah : 1;
-            maxp = max(maxp, __shfl_xor_sync(m4, maxp, 1));
-            maxp = max(maxp, __shfl_xor_sync(m4, maxp, 2));
+            if (STAGED) hme_task_layout(jb, jl, bw, bh, k, aligned, s_tpp, s_ntasks, s_kshift);
             if (jl) {
                 s_jobs[tid] = jb;
                 s_key[tid] = ~0ull;
-            }
-            if (tid == 0) {
-                s_tpp = tpp;
-                s_ntasks = tot;
-                // packed 32-bit keys when (largest SAD of the level, largest position index) fit together
-                const int ibits = 32 - __clz(maxp - 1 > 0 ? maxp - 1 : 1);
-                const int sbits = 32 - __clz(255 * bw * bh);
-                s_kshift = (ibits + sbits <= 31) ? ibits : 0;
             }
         }
         __syncthreads();
         const uint8_t *s = srcp + (size_t)(pl.origin_y + o_y) * pl.stride + pl.origin_x + o_x;
         const int sstr = sub ? pl.stride * 2 : pl.stride;
-        if (!aligned)
-            hme_level_search<NT_SEARCH>(s, sstr, pl.stride, k, bw, bh, s_jobs, njobs, smem, s_key);
-        else if (level == 0)
-            hme_level_search_aligned<NT_SEARCH, 4>(s, sstr, pl.stride, k, bh, s_jobs, njobs, s_tpp, s_ntasks, s_kshift, smem, s_key);
-        else if (level == 1)
-            hme_level_search_aligned<NT_SEARCH, 8>(s, sstr, pl.stride, k, bh, s_jobs, njobs, s_tpp, s_ntasks, s_kshift, smem, s_key);
-        else
-            hme_level_search_aligned<NT_SEARCH, 16>(s, sstr, pl.stride, k, bh, s_jobs, njobs, s_tpp, s_ntasks, s_kshift, smem, s_key);
+        if constexpr (STAGED) {
+            if (!aligned)
+                hme_level_search<NT_SEARCH>(s, sstr, pl.stride, k, bw, bh, s_jobs, njobs, smem, s_key);
+            else if (level == 0)
+                hme_level_search_aligned<NT_SEARCH, 4>(s, sstr, pl.stride, k, bh, s_jobs, njobs, s_tpp, s_ntasks, s_kshift, smem, s_key);
+            else if (level == 1)
+                hme_level_search_aligned<NT_SEARCH, 8>(s, sstr, pl.stride, k, bh, s_jobs, njobs, s_tpp, s_ntasks, s_kshift, smem, s_key);
+            else
+                hme_level_search_aligned<NT_SEARCH, 16>(s, sstr, pl.stride, k, bh, s_jobs, njobs, s_tpp, s_ntasks, s_kshift, smem, s_key);
+        } else {
+            __shared__ uint64_t s_red[NT_SEARCH / 32];
+            for (int j = 0; j < njobs; j++) {
+                const uint64_t key = block_search<NT_SEARCH>(s, sstr, s_jobs[j].ref, pl.stride, k, bw, bh, s_jobs[j].saw, s_jobs[j].sah,
+                                                             smem, HME_SMEM_BYTES, s_red);
+                if (tid == 0) s_key[j] = key;
+            }
+            __syncthreads();
+        }
         if (tid < njobs) {
             const unsigned long long key = s_key[tid];
             const uint32_t sad = (uint32_t)(key >> 32), idx = (uint32_t)key;
             int kx = 0, ky = 0;
-            unsigned long long lsad = 0xffffff; // svt_sad_loop_kernel_c start value
-            if (key != ~0ull && sad < 0xffffffu) {
+            unsigned long long lsad = 0xffffff; // svt_sad_loop_kernel_c start value; centre untouched if never beaten
+            if (sad < 0xffffffu) {
                 lsad = sad;
                 kx = idx % s_jobs[tid].saw;
                 ky = idx / s_jobs[tid].saw;
@@ -831,6 +739,8 @@ __global__ void __launch_bounds__(NT_SEARCH, 6) hme_kernel(const __grid_constant
         hme_publish(d, sb, out, w);
     }
 }
+__global__ void __launch_bounds__(NT_SEARCH, 6) hme_kernel_staged(const __grid_constant__ MeDev d) { hme_sb<true>(d); }
+__global__ void __launch_bounds__(NT_SEARCH) hme_kernel_chunked(const __grid_constant__ MeDev d) { hme_sb<false>(d); }
 
 // -----------------------------------------------------------------------------------------------------
 // SB epilogue: me_prune_ref (:2145-2199), construct_me_candidate_array (:2825-2905), MeSbResults (:2964-3040).
@@ -994,12 +904,10 @@ __global__ void __launch_bounds__(NT_SEARCH, 2) fullpel_kernel(const __grid_cons
     const uint8_t *refb = d.refs[l][r].full + (size_t)(fp.origin_y + oy) * fp.stride + fp.origin_x + ox;
 
     int xsc = hs.sc_x[l][r], ysc = hs.sc_y[l][r];
-    const int dist = scaled_dist(p.ref_dist[l][r]);
-    int saw = (int16_t)min(p.search_area_width * dist, p.max_me_search_width);
-    int sah = (int16_t)min(p.search_area_height * dist, p.max_me_search_height);
+    const int2 area = fp_search_area(p, scaled_dist(p.ref_dist[l][r]));
     const int dv = (int)hs.divisor[l][r];
-    saw = (int16_t)(((saw / dv) + 7) & ~0x07);
-    sah = (int16_t)max(1, sah / dv);
+    int saw = (int16_t)fp_window_width((int16_t)area.x / dv);
+    int sah = (int16_t)max(1, (int16_t)area.y / dv);
 
     // ---- stage the source rows that take part in the SAD (even rows only with sub-sampling) ----
     uint32_t *s_src = smem; // [NSRC][16 words]
@@ -1368,12 +1276,94 @@ __global__ void fill32_kernel(uint32_t *p, int n, uint32_t v) {
 static void set_attrs() {
     static PerDeviceOnce once;
     once.run([] {
-        SVTB_ATTR(hme_kernel_generic, HME_SMEM_BYTES);
-        SVTB_ATTR(hme_kernel, HME_FAST_SMEM);
+        SVTB_ATTR(hme_kernel_chunked, HME_SMEM_BYTES);
+        SVTB_ATTR(hme_kernel_staged, HME_FAST_SMEM);
         SVTB_ATTR(fullpel_kernel<true>, FP_SMEM_BYTES);
         SVTB_ATTR(fullpel_kernel<false>, FP_SMEM_BYTES);
         SVTB_ATTR(sad_loop_kernel, 200 * 1024);
     });
+}
+
+// The per-picture scratch: byte offsets of MeDev's raw[n_sb][2][4], hstate[n_sb], hme_done[n_sb] and fp_done[n_sb], and
+// the total.
+struct MeScratch {
+    size_t raw, hstate, hme_done, fp_done, bytes;
+};
+MeScratch me_scratch(const SvtB200MeParams &p) {
+    const size_t n_sb = (size_t)((p.full.width + 63) / 64) * ((p.full.height + 63) / 64);
+    MeScratch s;
+    s.raw = 0;
+    s.hstate = s.raw + n_sb * 8 * sizeof(RawHme);
+    s.hme_done = s.hstate + n_sb * sizeof(HmeState);
+    s.fp_done = s.hme_done + n_sb * sizeof(unsigned int);
+    s.bytes = s.fp_done + n_sb * sizeof(unsigned int);
+    return s;
+}
+
+// What svt_b200_me_picture launches for a picture with parameters `p` (validated): the HME regime, the dynamic shared
+// memory of the HME and full-pel kernels, and the full-pel CTA width.  Host arithmetic only.
+struct MeLaunchPlan {
+    bool hme_staged;
+    int hme_smem, fp_smem, fp_threads;
+};
+MeLaunchPlan me_launch_plan(const SvtB200MeParams &p) {
+    // per reference: the full-pel warp-tasks (32 tasks of 4 positions) of its whole search window
+    int maxd = 1, n = 0, warp_tasks[SVT_B200_ME_LISTS * SVT_B200_ME_MAX_REFS];
+    for (int l = 0; l < p.num_lists; l++)
+        for (int r = 0; r < p.num_refs[l]; r++) {
+            const int dd = scaled_dist(p.ref_dist[l][r]);
+            maxd = std::max(maxd, dd);
+            const int2 a = fp_search_area(p, dd);
+            warp_tasks[n++] = (a.y * 4 * ((fp_window_width(a.x) + 15) >> 4) + 31) / 32;
+        }
+    MeLaunchPlan plan;
+    { // worst-case shared memory of one HME level in the staged regime (4 windows + the source block)
+        const int k = p.hme_search_method ? 2 : 1;
+        auto level_bytes = [&](int saw, int sah, int bw, int bh) {
+            const int bhh = k == 2 ? bh / 2 : bh;
+            int wpw = ((saw - 1 + bw + 3) / 4) + 1;
+            wpw = std::max(wpw, std::max(hme_pitch_words(saw, bw / 4, 2), hme_pitch_words(saw, bw / 4, 4)));
+            const size_t win = (size_t)wpw * 4 * (sah - 1 + (bhh - 1) * k + 1);
+            return 4 * win + (size_t)((bw + 3) / 4) * 4 * bhh;
+        };
+        // the kernel indexes the per-region arrays with [rx] / [ry]: size for the largest region that is used, at the
+        // largest distance
+        const int nrx = p.number_hme_search_region_in_width, nry = p.number_hme_search_region_in_height;
+        auto amax = [](const int32_t *a, int n) { return n > 1 ? std::max(a[0], a[1]) : a[0]; };
+        int w0 = amax(p.hme_level0_search_area_in_width_array, nrx) * maxd, h0 = amax(p.hme_level0_search_area_in_height_array, nry) * maxd;
+        const int w0m = amax(p.hme_level0_max_search_area_in_width_array, nrx), h0m = amax(p.hme_level0_max_search_area_in_height_array, nry);
+        if (w0 > w0m) w0 = w0m;
+        if (h0 > h0m) h0 = h0m;
+        size_t a = level_bytes((w0 + 15) & ~15, h0, 16, 16);
+        size_t b = level_bytes((amax(p.hme_level1_search_area_in_width_array, nrx) + 7) & ~7, amax(p.hme_level1_search_area_in_height_array, nry), 32, 32);
+        size_t c = level_bytes((amax(p.hme_level2_search_area_in_width_array, nrx) + 7) & ~7, amax(p.hme_level2_search_area_in_height_array, nry), 64, 64);
+        size_t hme_need = a > b ? a : b;
+        hme_need = hme_need > c ? hme_need : c;
+        hme_need += 256;
+        plan.hme_staged = hme_need <= (size_t)HME_FAST_SMEM;
+        plan.hme_smem = plan.hme_staged ? (int)hme_need : HME_SMEM_BYTES;
+    }
+    { // the full-pel search: source rows + the largest window (whole if it fits)
+        const int2 a = fp_search_area(p, maxd);
+        const int saw = fp_window_width(a.x), sah = a.y;
+        const int sub = p.me_search_method != 0;
+        size_t need = (size_t)(sub ? 32 : 64) * 64 + (size_t)fp_pitch_words(saw) * 4 * (sah - 1 + (sub ? 63 : 64)) + 64;
+        if (need > (size_t)FP_SMEM_BYTES) need = FP_SMEM_BYTES;
+        plan.fp_smem = (int)need;
+    }
+    // full-pel CTA size: pick the warp count that divides the per-reference warp-task counts best (idle warps only hold
+    // registers until the CTA's last round ends)
+    static const int cand[5] = {4, 3, 6, 2, 8};
+    long best_cost = -1;
+    for (int ci = 0; ci < 5; ci++) {
+        long cost = 0;
+        for (int i = 0; i < n; i++) cost += (long)((warp_tasks[i] + cand[ci] - 1) / cand[ci]) * cand[ci];
+        if (best_cost < 0 || cost < best_cost) {
+            best_cost = cost;
+            plan.fp_threads = cand[ci] * 32;
+        }
+    }
+    return plan;
 }
 
 } // namespace
@@ -1382,8 +1372,7 @@ extern "C" {
 
 size_t svt_b200_me_scratch_bytes(const SvtB200MeParams *p) {
     if (!p) return 0;
-    const size_t n_sb = (size_t)((p->full.width + 63) / 64) * ((p->full.height + 63) / 64);
-    return n_sb * (8 * sizeof(RawHme) + sizeof(HmeState) + 2 * sizeof(unsigned int));
+    return me_scratch(*p).bytes;
 }
 
 int svt_b200_me_picture(const SvtB200MeParams *p, const SvtB200MePlanes *src,
@@ -1407,13 +1396,18 @@ int svt_b200_me_picture(const SvtB200MeParams *p, const SvtB200MePlanes *src,
         return SVT_B200_ERR_UNSUPPORTED;
     }
     set_attrs();
+    const MeLaunchPlan plan = me_launch_plan(*p);
+    const MeScratch sc = me_scratch(*p);
     MeDev d;
     memset(&d, 0, sizeof(d));
     d.p = *p;
     d.src = *src;
     memcpy(d.refs, refs, sizeof(d.refs));
     d.out = *out;
-    d.raw = (RawHme *)scratch;
+    d.raw = (RawHme *)((char *)scratch + sc.raw);
+    d.hstate = (HmeState *)((char *)scratch + sc.hstate);
+    d.hme_done = (unsigned int *)((char *)scratch + sc.hme_done);
+    d.fp_done = (unsigned int *)((char *)scratch + sc.fp_done);
     d.sbs_x = (p->full.width + 63) / 64;
     d.sbs_y = (p->full.height + 63) / 64;
     int n = 0;
@@ -1424,95 +1418,21 @@ int svt_b200_me_picture(const SvtB200MeParams *p, const SvtB200MePlanes *src,
             n++;
         }
     d.n_slots = n;
+    d.fp_smem_bytes = plan.fp_smem;
     const int n_sb = d.sbs_x * d.sbs_y;
     cudaStream_t st = (cudaStream_t)stream;
     // slots of unused references are defined as zero
     SVTB_CUDA_TRY(cudaMemsetAsync(out->best_sad, 0, (size_t)n_sb * 8 * 85 * 4, st));
     SVTB_CUDA_TRY(cudaMemsetAsync(out->best_mv, 0, (size_t)n_sb * 8 * 85 * 4, st));
-    d.hstate = (HmeState *)(d.raw + (size_t)n_sb * 8);
-    d.hme_done = (unsigned int *)(d.hstate + n_sb);
-    d.fp_done = d.hme_done + n_sb;
-    SVTB_CUDA_TRY(cudaMemsetAsync(d.raw, 0, (size_t)n_sb * (8 * sizeof(RawHme) + sizeof(HmeState) + 2 * sizeof(unsigned int)), st));
-    // worst-case shared memory of one HME level on the fast path (4 windows + the source block)
-    size_t hme_need = 0;
-    {
-        const int k = p->hme_search_method ? 2 : 1;
-        int maxd = 1;
-        for (int l = 0; l < p->num_lists; l++)
-            for (int r = 0; r < p->num_refs[l]; r++) {
-                int dd = p->ref_dist[l][r];
-                dd = ((dd * 5) / 8) + ((dd % 8) ? 1 : 0);
-                if (dd > maxd) maxd = dd;
-            }
-        auto level_bytes = [&](int saw, int sah, int bw, int bh) {
-            const int bhh = k == 2 ? bh / 2 : bh;
-            int wpw = ((saw - 1 + bw + 3) / 4) + 1;
-            wpw = std::max(wpw, std::max(hme_pitch_words(saw, bw / 4, 2), hme_pitch_words(saw, bw / 4, 4)));
-            const size_t win = (size_t)wpw * 4 * (sah - 1 + (bhh - 1) * k + 1);
-            return 4 * win + (size_t)((bw + 3) / 4) * 4 * bhh;
-        };
-        // the kernel indexes the per-region arrays with [rx] / [ry]: size for the largest region that is used
-        const int nrx = p->number_hme_search_region_in_width, nry = p->number_hme_search_region_in_height;
-        auto amax = [](const int32_t *a, int n) { return n > 1 ? std::max(a[0], a[1]) : a[0]; };
-        int w0 = amax(p->hme_level0_search_area_in_width_array, nrx) * maxd, h0 = amax(p->hme_level0_search_area_in_height_array, nry) * maxd;
-        const int w0m = amax(p->hme_level0_max_search_area_in_width_array, nrx), h0m = amax(p->hme_level0_max_search_area_in_height_array, nry);
-        if (w0 > w0m) w0 = w0m;
-        if (h0 > h0m) h0 = h0m;
-        size_t a = level_bytes((w0 + 15) & ~15, h0, 16, 16);
-        size_t b = level_bytes((amax(p->hme_level1_search_area_in_width_array, nrx) + 7) & ~7, amax(p->hme_level1_search_area_in_height_array, nry), 32, 32);
-        size_t c = level_bytes((amax(p->hme_level2_search_area_in_width_array, nrx) + 7) & ~7, amax(p->hme_level2_search_area_in_height_array, nry), 64, 64);
-        hme_need = a > b ? a : b;
-        hme_need = hme_need > c ? hme_need : c;
-        hme_need += 256;
-    }
-    if (hme_need <= (size_t)HME_FAST_SMEM)
-        SVTB_LAUNCH(hme_kernel, dim3(n_sb, n), NT_SEARCH, hme_need, st, d);
+    SVTB_CUDA_TRY(cudaMemsetAsync(scratch, 0, sc.bytes, st));
+    if (plan.hme_staged)
+        SVTB_LAUNCH(hme_kernel_staged, dim3(n_sb, n), NT_SEARCH, plan.hme_smem, st, d);
     else
-        SVTB_LAUNCH(hme_kernel_generic, dim3(n_sb, n), NT_SEARCH, HME_SMEM_BYTES, st, d);
-    int fp_threads = NT_SEARCH;
-    {   // shared memory of the full-pel search: source rows + the largest window (whole if it fits)
-        int maxd = 1;
-        for (int l = 0; l < p->num_lists; l++)
-            for (int r = 0; r < p->num_refs[l]; r++) {
-                int dd = p->ref_dist[l][r];
-                dd = ((dd * 5) / 8) + ((dd % 8) ? 1 : 0);
-                if (dd > maxd) maxd = dd;
-            }
-        int saw = p->search_area_width * maxd, sah = p->search_area_height * maxd;
-        if (saw > p->max_me_search_width) saw = p->max_me_search_width;
-        if (sah > p->max_me_search_height) sah = p->max_me_search_height;
-        saw = (saw + 7) & ~7;
-        const int sub = p->me_search_method != 0;
-        size_t need = (size_t)(sub ? 32 : 64) * 64 + (size_t)fp_pitch_words(saw) * 4 * (sah - 1 + (sub ? 63 : 64)) + 64;
-        if (need > (size_t)FP_SMEM_BYTES) need = FP_SMEM_BYTES;
-        d.fp_smem_bytes = (int)need;
-        // CTA size: a warp-task is 32 tasks of 4 positions; pick the warp count that divides the per-reference task
-        // counts best (idle warps only hold registers until the CTA's last round ends)
-        static const int cand[5] = {4, 3, 6, 2, 8};
-        long best_cost = -1;
-        for (int ci = 0; ci < 5; ci++) {
-            long cost = 0;
-            for (int l = 0; l < p->num_lists; l++)
-                for (int r = 0; r < p->num_refs[l]; r++) {
-                    int dd = p->ref_dist[l][r];
-                    dd = ((dd * 5) / 8) + ((dd % 8) ? 1 : 0);
-                    int w = p->search_area_width * dd, h = p->search_area_height * dd;
-                    if (w > p->max_me_search_width) w = p->max_me_search_width;
-                    if (h > p->max_me_search_height) h = p->max_me_search_height;
-                    w = (w + 7) & ~7;
-                    const int tw = (h * 4 * ((w + 15) >> 4) + 31) / 32;
-                    cost += (long)((tw + cand[ci] - 1) / cand[ci]) * cand[ci];
-                }
-            if (best_cost < 0 || cost < best_cost) {
-                best_cost = cost;
-                fp_threads = cand[ci] * 32;
-            }
-        }
-    }
+        SVTB_LAUNCH(hme_kernel_chunked, dim3(n_sb, n), NT_SEARCH, plan.hme_smem, st, d);
     if (p->me_search_method != 0)
-        SVTB_LAUNCH(fullpel_kernel<true>, dim3(n_sb, n), fp_threads, d.fp_smem_bytes, st, d);
+        SVTB_LAUNCH(fullpel_kernel<true>, dim3(n_sb, n), plan.fp_threads, plan.fp_smem, st, d);
     else
-        SVTB_LAUNCH(fullpel_kernel<false>, dim3(n_sb, n), fp_threads, d.fp_smem_bytes, st, d);
+        SVTB_LAUNCH(fullpel_kernel<false>, dim3(n_sb, n), plan.fp_threads, plan.fp_smem, st, d);
     SVTB_CUDA_TRY(cudaGetLastError());
     return SVT_B200_OK;
 }

@@ -1,5 +1,5 @@
 """GPU parity for motion estimation at the search windows of every preset (svtb200.me_params), bit-exact against the
-CPU oracle: the chunked full-pel search, the full-pel shared-memory clamp, the generic HME kernel, the launcher's
+CPU oracle: the chunked full-pel search, the full-pel shared-memory clamp, the chunked HME regime, the launcher's
 CTA widths and the full-SAD search, each with a host-side check that the case really takes the path it is named
 after.  test_oracle_me_presets.py pins the oracle against the reference on the same windows."""
 import ctypes as C
@@ -50,8 +50,8 @@ def used_refs(p):
 
 def launch_plan(p):
     """The kernel choices svt_b200_me_picture makes for `p`, with the launcher's own formulas: whether HME takes
-    hme_kernel_generic, the full-pel kernel's shared memory (and whether it was clamped to FP_SMEM_BYTES) and its
-    CTA width in warps."""
+    the chunked regime (hme_kernel_chunked), the full-pel kernel's shared memory (and whether it was clamped to
+    FP_SMEM_BYTES) and its CTA width in warps."""
     maxd = max([1] + [scaled_dist(p.ref_dist[l][r]) for l, r in used_refs(p)])
     k = 2 if p.hme_search_method else 1
 
@@ -187,13 +187,13 @@ def test_me_chunk_merge_keeps_first_tie(preset, chunks):
     (1, ((16, 2, 0, 0), (8, 0, 0, 0)), None, 200, 136),      # 60 * 10, capped at 240
     (1, ((1, 1, 0, 0), (1, 0, 0, 0)), sb.RES_4K, 320, 192),  # the 4K-class table: 120 per region at distance 1
 ])
-def test_me_generic_hme_kernel(preset, dist, res_class, w, h):
-    """hme_kernel_generic: the fast HME path's shared-memory need exceeds HME_FAST_SMEM."""
+def test_me_chunked_hme_kernel(preset, dist, res_class, w, h):
+    """hme_kernel_chunked, the chunked HME regime: the staged regime's shared-memory need exceeds HME_FAST_SMEM."""
     params = sb.me_params(preset, w, h, 2, 1, dist, 1, 1, input_resolution_class=res_class)
     plan = launch_plan(params)
     assert plan["hme_generic"] and plan["hme_need"] > HME_FAST_SMEM
     assert plan["w0"] >= (120 if res_class is not None else 180)
-    gpu_vs_oracle(params, cm.make_me_case(w, h, 2, 1, seed=80 + preset), f"generic HME preset {preset}")
+    gpu_vs_oracle(params, cm.make_me_case(w, h, 2, 1, seed=80 + preset), f"chunked HME preset {preset}")
 
 
 # (preset, reference distances, n_l0, n_l1, the full-pel CTA width in warps that the launcher picks for them)
@@ -258,7 +258,7 @@ def _engine_me(lib, e, params, src, refs, n_sb):
 
 
 def test_engine_me_picture_at_preset1_windows():
-    """The engine's slot staging passes preset 1's windows (generic HME, 192-wide full-pel windows) through: its
+    """The engine's slot staging passes preset 1's windows (chunked HME, 192-wide full-pel windows) through: its
     outputs equal the direct entry's."""
     import gpu_runner as gr
     from test_engine_gpu import assert_me_result
