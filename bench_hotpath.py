@@ -776,7 +776,7 @@ def roofline(stage_ms, pk, pk_kind, n_sb):
     bound = {"me": "integer ALU / shared memory (VABSDIFF4 issue rate)", "encdec": "shared-memory butterflies, then HBM",
              "dlf": "hbm", "cdef_search": "integer ALU (10 filters per sample)", "cdef_apply": "hbm"}
     kernels = {"me": ("hme_kernel", "fullpel_kernel"), "encdec": ("encode_tu_kernel",), "dlf": ("dlf_vert_kernel", "dlf_horz_kernel"),
-               "cdef_search": ("cdef_search_grid_kernel",), "cdef_apply": ("cdef_apply_kernel",)}
+               "cdef_search": ("cdef_search_kernel",), "cdef_apply": ("cdef_apply_kernel",)}
     stages = []
     for k, b in alg.items():
         ach = b / (stage_ms[k] / 1e3) / 1e9

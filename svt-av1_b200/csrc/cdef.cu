@@ -6,12 +6,14 @@
 //   compute_cdef_dist_c / _8bit_c (incl. the double-precision 8x8 distortion) Encoder/Codec/EbEncCdef.c:20-220
 //   svt_av1_cdef_frame / av1_cdef_frame16bit                           Encoder/Codec/EbEncCdef.c:292-1030
 //
-// Design: one CTA per 64x64 filter block.  The deblocked reconstruction of the block (+2 sample rim, frame
-// exterior = CDEF_VERY_LARGE) is staged ONCE into shared memory as int16 and every strength of the search is
-// evaluated from that tile, so HBM traffic is recon + source once per block (2 B/sample, SURVEY §8d) instead
-// of once per strength.  A thread owns one row of one 8x8 (or 4x4 chroma) block; block sums for the
-// distortion are reduced with 8-lane shuffles.  The 8x8 luma distortion keeps the reference's double formula
-// with explicit round-to-nearest intrinsics (no FMA contraction) so it is bit-identical (0 ULP).
+// Design: the strength search runs two CTAs per 64x64 filter block, one for luma and one for both chroma planes (it
+// stages the luma tile too, for the block directions).  Each plane of the deblocked reconstruction of the block (+2
+// sample rim, frame exterior = CDEF_VERY_LARGE) is staged ONCE into shared memory as int16 and every strength of the
+// search is evaluated from that tile, so HBM traffic is recon + source once per block (2 B/sample, SURVEY §8d) instead
+// of once per strength.  One kernel body has two search forms: the separable form for the pri x sec grids that every
+// encoder table is (plane_search_grid), and one pass per strength for any other list (plane_search_list).  The apply
+// runs one CTA per filter block.  The 8x8 luma distortion keeps the reference's double formula with explicit
+// round-to-nearest intrinsics (no FMA contraction) so it is bit-identical (0 ULP).
 #include <algorithm>
 
 #include "common.cuh"
@@ -41,57 +43,28 @@ __device__ __forceinline__ int adjust_strength(int strength, int var) {
     return var ? (strength * (4 + i) + 8) >> 4 : 0;
 }
 
-// body of svt_cdef_filter_block_c for one sample; `in` points into an int16 tile of stride `s`
-__device__ __forceinline__ int cdef_sample(const int16_t *in, int s, int pri, int sec, int dir, int pri_damping,
-                                           int sec_damping, int coeff_shift) {
-    const int x = in[0];
-    if (pri == 0 && sec == 0) return x; // every constrain() is 0 and x lies inside [min,max]
-    const int odd = (pri >> coeff_shift) & 1;
-    const int pt0 = odd ? 3 : 4, pt1 = odd ? 3 : 2;
-    const int psh = pri ? max(0, pri_damping - msb((uint32_t)pri)) : 0;
-    const int ssh = sec ? max(0, sec_damping - msb((uint32_t)sec)) : 0;
-    int sum = 0, mx = x, mn = x;
+// Tile offsets of the primary taps (direction dir) and the secondary taps (dir +/- 2) in a tile of row stride s
+__device__ __forceinline__ void tap_offsets(int dir, int s, int (&po)[2], int (&o2)[2], int (&o6)[2]) {
 #pragma unroll
     for (int k = 0; k < 2; k++) {
-        const int po = c_dir[dir][k][0] * s + c_dir[dir][k][1];
-        const int p0 = in[po], p1 = in[-po];
-        const int pt = k ? pt1 : pt0;
-        if (pri) sum += pt * constrain_s(p0 - x, pri, psh) + pt * constrain_s(p1 - x, pri, psh);
-        if (p0 != VERY_LARGE) mx = max(mx, p0);
-        if (p1 != VERY_LARGE) mx = max(mx, p1);
-        mn = min(mn, min(p0, p1));
-        const int o2 = c_dir[(dir + 2) & 7][k][0] * s + c_dir[(dir + 2) & 7][k][1];
-        const int o6 = c_dir[(dir + 6) & 7][k][0] * s + c_dir[(dir + 6) & 7][k][1];
-        const int s0 = in[o2], s1 = in[-o2], s2 = in[o6], s3 = in[-o6];
-        if (s0 != VERY_LARGE) mx = max(mx, s0);
-        if (s1 != VERY_LARGE) mx = max(mx, s1);
-        if (s2 != VERY_LARGE) mx = max(mx, s2);
-        if (s3 != VERY_LARGE) mx = max(mx, s3);
-        mn = min(mn, min(min(s0, s1), min(s2, s3)));
-        const int stp = k ? 1 : 2;
-        if (sec)
-            sum += stp * (constrain_s(s0 - x, sec, ssh) + constrain_s(s1 - x, sec, ssh) + constrain_s(s2 - x, sec, ssh) +
-                          constrain_s(s3 - x, sec, ssh));
+        po[k] = c_dir[dir][k][0] * s + c_dir[dir][k][1];
+        o2[k] = c_dir[(dir + 2) & 7][k][0] * s + c_dir[(dir + 2) & 7][k][1];
+        o6[k] = c_dir[(dir + 6) & 7][k][0] * s + c_dir[(dir + 6) & 7][k][1];
     }
-    const int y = x + ((8 + sum - (sum < 0)) >> 4);
-    return min(max(y, mn), mx);
 }
 
-// Search-kernel variant of cdef_sample with everything that is constant over a block hoisted by the caller:
-// tap offsets for the block's direction, damping shifts, tap weights.  kBorder = false is used for filter blocks
-// that do not touch the frame edge (no CDEF_VERY_LARGE samples in the tile): the "!= VERY_LARGE" tests vanish.
+// svt_cdef_filter_block_c for one sample, with everything that is constant over a block hoisted into CdefTaps by the
+// caller: tap offsets for the block's direction, damping shifts, tap weights.  `in` points into an int16 tile of the row
+// stride `s` given to make_taps.  kBorder = false is used for filter blocks that do not touch the frame edge (no
+// CDEF_VERY_LARGE samples in the tile): the "!= VERY_LARGE" tests vanish.  For pri == sec == 0 the result is x, which
+// lies inside [min, max].
 struct CdefTaps {
     int po[2], o2[2], o6[2];
     int pt0, pt1, psh, ssh;
 };
 __device__ __forceinline__ CdefTaps make_taps(int pri, int sec, int dir, int pri_damping, int sec_damping, int coeff_shift, int s) {
     CdefTaps t;
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-        t.po[k] = c_dir[dir][k][0] * s + c_dir[dir][k][1];
-        t.o2[k] = c_dir[(dir + 2) & 7][k][0] * s + c_dir[(dir + 2) & 7][k][1];
-        t.o6[k] = c_dir[(dir + 6) & 7][k][0] * s + c_dir[(dir + 6) & 7][k][1];
-    }
+    tap_offsets(dir, s, t.po, t.o2, t.o6);
     const int odd = (pri >> coeff_shift) & 1;
     t.pt0 = odd ? 3 : 4;
     t.pt1 = odd ? 3 : 2;
@@ -244,10 +217,6 @@ struct FrameDev {
     int stride[3];
     int hbd;
 };
-template <typename T>
-__device__ __forceinline__ int ldpx(const void *p, size_t off) {
-    return reinterpret_cast<const T *>(p)[off];
-}
 
 // Stage the filter block of plane `pli` (+2 rim; outside the frame = VERY_LARGE) into an int16 tile.  Work item = four
 // horizontally adjacent samples starting at a frame x that is a multiple of 4 (tile columns 4g-2 .. 4g+1, written as
@@ -302,14 +271,101 @@ __device__ void load_tile(const void *plane_v, int stride, int pw, int ph, int y
     }
 }
 
+// 64x64 filter blocks (16x16 4x4 units) per picture column or row of `mi` 4x4 units
+static int fb_count(int mi) { return (mi + 15) / 16; }
+
+// One plane's part of a filter block, in samples of that plane
+struct PlaneRect {
+    int pw, ph; // plane size
+    int bh, bw; // block size, clipped to the plane
+    int y0, x0; // block origin
+};
+// The filter block of CTA x index `fb` (raster order, nhfb per row) in a picture of mi_rows x mi_cols 4x4 units
+struct FilterBlock {
+    int mi_rows, mi_cols;
+    int fbr, fbc; // row and column in filter blocks
+    int nvb, nhb; // size in 4x4 units, clipped to the picture
+    int border; // nonzero when the +2 rim reaches outside the frame (CDEF_VERY_LARGE samples present); an int, as a bool
+                // member costs cdef_apply_kernel 8 registers
+    __device__ FilterBlock(int fb, int nhfb, int mi_rows_, int mi_cols_) : mi_rows(mi_rows_), mi_cols(mi_cols_) {
+        fbr = fb / nhfb;
+        fbc = fb - fbr * nhfb;
+        nvb = min(16, mi_rows - 16 * fbr);
+        nhb = min(16, mi_cols - 16 * fbc);
+        border = fbr == 0 || fbc == 0 || 16 * (fbr + 1) >= mi_rows || 16 * (fbc + 1) >= mi_cols;
+    }
+    __device__ PlaneRect plane(int pli) const {
+        const int sh = pli ? 1 : 0;
+        return {(mi_cols * 4) >> sh, (mi_rows * 4) >> sh, (nvb * 4) >> sh, (nhb * 4) >> sh, (fbr * 64) >> sh, (fbc * 64) >> sh};
+    }
+};
+// Stage plane `pli` of the filter block from `f` into `tile`, between two barriers: the first one waits until every
+// thread is done with the previous plane's tile.
+template <typename T>
+__device__ __forceinline__ PlaneRect stage_plane(const FilterBlock &fb, const FrameDev &f, int pli, int16_t *tile) {
+    const PlaneRect r = fb.plane(pli);
+    __syncthreads();
+    load_tile<T>(f.p[pli], f.stride[pli], r.pw, r.ph, r.y0, r.x0, r.bh, r.bw, tile);
+    __syncthreads();
+    return r;
+}
+
+// Strengths of the search's separable form (see plane_search_grid): entry gi = pi * NSEC + si is (pri[pi], sec[si])
+struct CdefGrid {
+    int npri;
+    int pri[16], sec[4];
+};
 struct CdefSearchDev {
     SvtB200CdefSearchParams p;
+    CdefGrid g; // read by the grid instances only
     FrameDev recon, source;
     const uint8_t *skip8;
     int skip_stride;
     uint64_t *mse;
     int nvfb, nhfb, coeff_shift;
 };
+
+// svt_sb_compute_cdef_list: raster list of the filter block's non-skip 8x8 blocks into s_by, s_bx (warp 0, two blocks per
+// lane, ballots).  Ends with a barrier and returns the count to every thread.
+__device__ __forceinline__ int block_list(const FilterBlock &fb, const uint8_t *skip8, int skip_stride, uint8_t *s_by, uint8_t *s_bx) {
+    __shared__ int s_count;
+    const int tid = threadIdx.x;
+    if (tid < 32) {
+        unsigned int m[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int b = tid + 32 * h, r = (b >> 3) * 2, c = (b & 7) * 2;
+            const bool on = r < fb.nvb && c < fb.nhb && !skip8[(size_t)((16 * fb.fbr + r) >> 1) * skip_stride + ((16 * fb.fbc + c) >> 1)];
+            m[h] = __ballot_sync(0xffffffffu, on);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+            if ((m[h] >> tid) & 1u) {
+                const int n = (h ? __popc(m[0]) : 0) + __popc(m[h] & ((1u << tid) - 1u));
+                s_by[n] = (uint8_t)((tid + 32 * h) >> 3);
+                s_bx[n] = (uint8_t)(tid & 7);
+            }
+        if (tid == 0) s_count = __popc(m[0]) + __popc(m[1]);
+    }
+    __syncthreads();
+    return s_count;
+}
+
+// Write plane `pli`'s 64 entries of this filter block's mse row from the sums in s_mse, and clear s_mse for the next plane.
+// The two chroma planes share a row.  Entries past n_strengths, and every entry of an all-skip filter block (count 0,
+// svt_sb_all_skip: not searched), are 0.
+__device__ __forceinline__ void store_mse(const CdefSearchDev &d, int pli, int count, unsigned long long *s_mse) {
+    uint64_t *out = d.mse + ((pli ? (size_t)d.nvfb * d.nhfb : 0) + blockIdx.x) * 64;
+    for (int gi = threadIdx.x; gi < 64; gi += NT) {
+        unsigned long long v = 0;
+        if (count && gi < d.p.n_strengths) v = s_mse[gi] >> (2 * d.coeff_shift);
+        s_mse[gi] = 0;
+        if (pli == 2)
+            out[gi] += v;
+        else
+            out[gi] = v;
+    }
+}
 
 // dist_8x8_8bit_c / dist_8x8_16bit_c (EbEncCdef.c:20-33, 75-98): identical IEEE double operation sequence
 __device__ __forceinline__ unsigned long long dist8x8_from_sums(unsigned long long sum_s, unsigned long long sum_d,
@@ -323,126 +379,69 @@ __device__ __forceinline__ unsigned long long dist8x8_from_sums(unsigned long lo
     return (unsigned long long)floor(__dadd_rn(.5, __ddiv_rn(b, c)));
 }
 
+// ---- search, list form --------------------------------------------------------------------------------------------
+// Any strength list: one pass over the listed blocks per strength.  A thread owns one row of one 8x8 (or 4x4 chroma) block.
 template <typename T>
-__global__ void __launch_bounds__(NT) cdef_search_kernel(const __grid_constant__ CdefSearchDev d) {
-    __shared__ int16_t tile[68 * TS];
-    __shared__ uint8_t s_by[64], s_bx[64];
-    __shared__ int8_t s_dir[64];
-    __shared__ int s_var[64];
-    __shared__ int s_count;
-    __shared__ unsigned long long s_mse[64];
-    const int tid = threadIdx.x;
-    const int fb = blockIdx.x, fbr = fb / d.nhfb, fbc = fb - fbr * d.nhfb;
+__device__ __forceinline__ int ldpx(const void *p, size_t off) {
+    return reinterpret_cast<const T *>(p)[off];
+}
+template <typename T>
+__device__ __forceinline__ void plane_search_list(const CdefSearchDev &d, const int16_t *in, int count, const uint8_t *s_by,
+                                                  const uint8_t *s_bx, const int8_t *s_dir, const int *s_var, unsigned long long *s_mse,
+                                                  int pli, int y0, int x0, int damping, bool border) {
+    const int tid = threadIdx.x, bs = pli ? 4 : 8, cs = d.coeff_shift;
     const SvtB200CdefSearchParams &p = d.p;
-    const int nvb = min(16, p.mi_rows - 16 * fbr), nhb = min(16, p.mi_cols - 16 * fbc);
-    const int cs = d.coeff_shift;
-    // does the +2 rim of this filter block reach outside the frame (CDEF_VERY_LARGE samples present)?
-    const bool border = fbr == 0 || fbc == 0 || 16 * (fbr + 1) >= p.mi_rows || 16 * (fbc + 1) >= p.mi_cols;
-    uint64_t *out_y = d.mse + ((size_t)fb) * 64;
-    uint64_t *out_c = d.mse + ((size_t)d.nvfb * d.nhfb + fb) * 64;
-    if (tid < 32) { // svt_sb_compute_cdef_list: raster list of the non-skip 8x8 blocks (two blocks per lane, ballots)
-        unsigned int m[2];
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const int b = tid + 32 * h, r = (b >> 3) * 2, c = (b & 7) * 2;
-            const bool on = r < nvb && c < nhb && !d.skip8[(size_t)((16 * fbr + r) >> 1) * d.skip_stride + ((16 * fbc + c) >> 1)];
-            m[h] = __ballot_sync(0xffffffffu, on);
-        }
-#pragma unroll
-        for (int h = 0; h < 2; h++)
-            if ((m[h] >> tid) & 1u) {
-                const int n = (h ? __popc(m[0]) : 0) + __popc(m[h] & ((1u << tid) - 1u));
-                s_by[n] = (uint8_t)((tid + 32 * h) >> 3);
-                s_bx[n] = (uint8_t)(tid & 7);
-            }
-        if (tid == 0) s_count = __popc(m[0]) + __popc(m[1]);
-    }
-    __syncthreads();
-    const int count = s_count;
-    if (count == 0) { // svt_sb_all_skip: not searched; entries defined as 0
-        for (int i = tid; i < 64; i += NT) {
-            out_y[i] = 0;
-            out_c[i] = 0;
-        }
-        return;
-    }
-    for (int pli = 0; pli < 3; pli++) {
-        const int sh = pli ? 1 : 0, bs = 8 >> sh;
-        const int pw = (p.mi_cols * 4) >> sh, ph = (p.mi_rows * 4) >> sh;
-        const int bh = (nvb * 4) >> sh, bw = (nhb * 4) >> sh;
-        const int y0 = (fbr * 64) >> sh, x0 = (fbc * 64) >> sh;
-        __syncthreads();
-        load_tile<T>(d.recon.p[pli], d.recon.stride[pli], pw, ph, y0, x0, bh, bw, tile);
-        for (int i = tid; i < 64; i += NT) s_mse[i] = 0;
-        __syncthreads();
-        const int16_t *in = tile + 2 * TS + 2;
-        if (pli == 0) {
-            find_dirs(in, s_by, s_bx, count, cs, s_dir, s_var);
-            __syncthreads();
-        }
-        const int damping = p.pri_damping + cs - (pli != 0);
-        const int rows_per_blk = bs; // threads per block = rows
-        const int blk_per_pass = NT / rows_per_blk;
-        const void *sp = d.source.p[pli];
-        const int sstride = d.source.stride[pli];
-        for (int gi = 0; gi < p.n_strengths; gi++) {
-            const int pri = p.pri_strength[gi] << cs, sec = p.sec_strength[gi] << cs;
-            unsigned long long acc = 0;
-            for (int b0 = 0; b0 < count; b0 += blk_per_pass) {
-                const int b = b0 + tid / rows_per_blk, row = tid % rows_per_blk;
-                const bool live = b < count;
-                unsigned int ss = 0, sd = 0, ss2 = 0, sd2 = 0, ssd = 0, se = 0;
-                if (live) {
-                    const int by = s_by[b], bx = s_bx[b];
-                    const int t = pli ? pri : adjust_strength(pri, s_var[b]);
-                    const int dir = pri ? s_dir[b] : 0;
-                    const int16_t *q = in + (by * bs + row) * TS + bx * bs;
-                    const size_t so = (size_t)(y0 + by * bs + row) * sstride + x0 + bx * bs;
-                    const bool ident = t == 0 && sec == 0;
-                    const CdefTaps taps = make_taps(t, sec, dir, damping, damping, cs, TS);
-                    for (int j = 0; j < bs; j++) {
-                        const int f = ident ? (int)q[j] : (border ? cdef_px<true>(q + j, taps, t, sec) : cdef_px<false>(q + j, taps, t, sec));
-                        const int o = ldpx<T>(sp, so + j);
-                        if (pli == 0) {
-                            ss += f;
-                            sd += o;
-                            ss2 += f * f;
-                            sd2 += o * o;
-                            ssd += f * o;
-                        } else {
-                            se += (o - f) * (o - f);
-                        }
+    const int rows_per_blk = bs; // threads per block = rows
+    const int blk_per_pass = NT / rows_per_blk;
+    const void *sp = d.source.p[pli];
+    const int sstride = d.source.stride[pli];
+    for (int gi = 0; gi < p.n_strengths; gi++) {
+        const int pri = p.pri_strength[gi] << cs, sec = p.sec_strength[gi] << cs;
+        unsigned long long acc = 0;
+        for (int b0 = 0; b0 < count; b0 += blk_per_pass) {
+            const int b = b0 + tid / rows_per_blk, row = tid % rows_per_blk;
+            const bool live = b < count;
+            unsigned int ss = 0, sd = 0, ss2 = 0, sd2 = 0, ssd = 0, se = 0;
+            if (live) {
+                const int by = s_by[b], bx = s_bx[b];
+                const int t = pli ? pri : adjust_strength(pri, s_var[b]);
+                const int dir = pri ? s_dir[b] : 0;
+                const int16_t *q = in + (by * bs + row) * TS + bx * bs;
+                const size_t so = (size_t)(y0 + by * bs + row) * sstride + x0 + bx * bs;
+                const bool ident = t == 0 && sec == 0;
+                const CdefTaps taps = make_taps(t, sec, dir, damping, damping, cs, TS);
+                for (int j = 0; j < bs; j++) {
+                    const int f = ident ? (int)q[j] : (border ? cdef_px<true>(q + j, taps, t, sec) : cdef_px<false>(q + j, taps, t, sec));
+                    const int o = ldpx<T>(sp, so + j);
+                    if (pli == 0) {
+                        ss += f;
+                        sd += o;
+                        ss2 += f * f;
+                        sd2 += o * o;
+                        ssd += f * o;
+                    } else {
+                        se += (o - f) * (o - f);
                     }
                 }
-                if (pli == 0) { // 8 lanes = one 8x8 block
-#pragma unroll
-                    for (int o = 1; o < 8; o <<= 1) {
-                        ss += __shfl_xor_sync(0xffffffffu, ss, o);
-                        sd += __shfl_xor_sync(0xffffffffu, sd, o);
-                        ss2 += __shfl_xor_sync(0xffffffffu, ss2, o);
-                        sd2 += __shfl_xor_sync(0xffffffffu, sd2, o);
-                        ssd += __shfl_xor_sync(0xffffffffu, ssd, o);
-                    }
-                    if (live && row == 0) acc += dist8x8_from_sums(ss, sd, ss2, sd2, ssd, cs);
-                } else {
-                    acc += se;
-                }
             }
-            // CTA-wide sum of this strength
+            if (pli == 0) { // 8 lanes = one 8x8 block
 #pragma unroll
-            for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-            if ((tid & 31) == 0 && acc) atomicAdd(&s_mse[gi], acc);
+                for (int o = 1; o < 8; o <<= 1) {
+                    ss += __shfl_xor_sync(0xffffffffu, ss, o);
+                    sd += __shfl_xor_sync(0xffffffffu, sd, o);
+                    ss2 += __shfl_xor_sync(0xffffffffu, ss2, o);
+                    sd2 += __shfl_xor_sync(0xffffffffu, sd2, o);
+                    ssd += __shfl_xor_sync(0xffffffffu, ssd, o);
+                }
+                if (live && row == 0) acc += dist8x8_from_sums(ss, sd, ss2, sd2, ssd, cs);
+            } else {
+                acc += se;
+            }
         }
-        __syncthreads();
-        for (int gi = tid; gi < 64; gi += NT) {
-            const unsigned long long v = gi < p.n_strengths ? (s_mse[gi] >> (2 * cs)) : 0;
-            if (pli == 0)
-                out_y[gi] = v;
-            else if (pli == 1)
-                out_c[gi] = v;
-            else
-                out_c[gi] += v;
-        }
+        // CTA-wide sum of this strength
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        if ((tid & 31) == 0 && acc) atomicAdd(&s_mse[gi], acc);
     }
 }
 
@@ -453,29 +452,14 @@ __global__ void __launch_bounds__(NT) cdef_search_kernel(const __grid_constant__
 // direction set (direction 0 for the pri == 0 entries — `t ? dir : 0` in svt_cdef_filter_fb — and the block's
 // direction for the rest) and P once per primary strength: for the 5x2 table of preset 8 that is 32 constrain()
 // evaluations per pixel instead of 72, 24 tile loads instead of 108.
-struct CdefGrid {
-    int npri, nsec;
-    int pri[16], sec[4];
-};
-struct CdefSearchGridDev {
-    CdefSearchDev d;
-    CdefGrid g;
-};
-
 constexpr int CDEF_COMPACT_NG = 20; // strength tables up to this size park the per-block sums for a compact distortion pass
-// Build variants: (256,3) / (256,2) launch bounds and a force-inlined plane_search_grid remove most of the stack frame
-// but were slower when measured - the kernel lives on 4 resident CTAs per SM hiding the constrain() ALU chains.  The
-// CDEF_SEARCH_MINB / CDEF_SEARCH_INLINE switches below rebuild them for a comparison on the GPU at hand.
-#ifndef CDEF_SEARCH_MINB
-#define CDEF_SEARCH_MINB 4 // resident CTAs per SM the search kernel is compiled for (register cap 65536 / (256 * MINB))
-#endif
-#ifndef CDEF_SEARCH_INLINE
-#define CDEF_SEARCH_INLINE __noinline__
-#endif
+// Not inlined, and the grid instances of the search kernel are built for 4 resident CTAs per SM: a force-inlined
+// plane_search_grid and (256,3) / (256,2) launch bounds remove most of the stack frame but were slower when measured - the
+// kernel lives on 4 resident CTAs per SM hiding the constrain() ALU chains.
 template <typename T, int BS, int NSEC, bool LUMA, bool kBorder>
-__device__ CDEF_SEARCH_INLINE void plane_search_grid(const CdefSearchDev &d, const CdefGrid &g, const int16_t *in, int count,
-                                                  const uint8_t *s_by, const uint8_t *s_bx, const int8_t *s_dir, const int *s_var,
-                                                  unsigned long long *s_mse, uint32_t *s_sums, int pli, int y0, int x0, int damping) {
+__device__ __noinline__ void plane_search_grid(const CdefSearchDev &d, const CdefGrid &g, const int16_t *in, int count,
+                                               const uint8_t *s_by, const uint8_t *s_bx, const int8_t *s_dir, const int *s_var,
+                                               unsigned long long *s_mse, uint32_t *s_sums, int pli, int y0, int x0, int damping) {
     const int tid = threadIdx.x, lane = tid & 31;
     const int ng = g.npri * NSEC;
     // The 8x8 luma distortion is ~100 double-precision instructions evaluated by ONE lane per block: inside the strength
@@ -524,12 +508,7 @@ __device__ CDEF_SEARCH_INLINE void plane_search_grid(const CdefSearchDev &d, con
             if (want != have) { // uniform over the CTA
                 have = want;
                 int o2[2], o6[2], po[2];
-#pragma unroll
-                for (int k = 0; k < 2; k++) {
-                    po[k] = c_dir[dir][k][0] * TS + c_dir[dir][k][1];
-                    o2[k] = c_dir[(dir + 2) & 7][k][0] * TS + c_dir[(dir + 2) & 7][k][1];
-                    o6[k] = c_dir[(dir + 6) & 7][k][0] * TS + c_dir[(dir + 6) & 7][k][1];
-                }
+                tap_offsets(dir, TS, po, o2, o6);
 #pragma unroll
                 for (int j = 0; j < PX; j++) {
                     int tp[12];
@@ -641,89 +620,51 @@ __device__ CDEF_SEARCH_INLINE void plane_search_grid(const CdefSearchDev &d, con
     }
 }
 
+// NSEC = 2, 4: a grid table (plane_search_grid); NSEC = 0: any strength list (plane_search_list).
+// grid.y = 2: CTA (fb, 0) searches the luma plane, CTA (fb, 1) both chroma planes (it stages the luma tile once more for
+// the block directions).  One CTA per filter block was 510 CTAs = 0.86 waves at 1080p (ncu launch__waves_per_multiprocessor)
+// with every CTA a serial chain over three planes; split, the grid is 1020 CTAs of 2/3 and 1/3 of that chain.
 template <typename T, int NSEC>
-__global__ void __launch_bounds__(NT, CDEF_SEARCH_MINB) cdef_search_grid_kernel(const __grid_constant__ CdefSearchGridDev gd) {
+__global__ void __launch_bounds__(NT, 4) cdef_search_kernel(const __grid_constant__ CdefSearchDev d) {
     __shared__ int16_t tile[68 * TS];
     __shared__ uint8_t s_by[64], s_bx[64];
     __shared__ int8_t s_dir[64];
     __shared__ int s_var[64];
-    __shared__ int s_count;
     __shared__ unsigned long long s_mse[64];
-    __shared__ uint32_t s_sums[64 * CDEF_COMPACT_NG * 3 + 128]; // parked (sum f, sum f^2, sum f*o) per (block, strength) + (sum o, sum o^2)
-    const CdefSearchDev &d = gd.d;
-    const int tid = threadIdx.x;
-    // grid.y = 2: CTA (fb, 0) searches the luma plane, CTA (fb, 1) both chroma planes (it stages the luma tile once more for
-    // the block directions).  One CTA per filter block was 510 CTAs = 0.86 waves at 1080p (ncu launch__waves_per_multiprocessor)
-    // with every CTA a serial chain over three planes; split, the grid is 1020 CTAs of 2/3 and 1/3 of that chain.
-    const int fb = blockIdx.x, fbr = fb / d.nhfb, fbc = fb - fbr * d.nhfb;
+    __shared__ uint32_t s_sums[NSEC ? 64 * CDEF_COMPACT_NG * 3 + 128 : 1]; // parked (sum f, sum f^2, sum f*o) per (block, strength) + (sum o, sum o^2)
+    const FilterBlock fb(blockIdx.x, d.nhfb, d.p.mi_rows, d.p.mi_cols);
     const bool chroma_cta = blockIdx.y != 0;
-    const SvtB200CdefSearchParams &p = d.p;
-    const int nvb = min(16, p.mi_rows - 16 * fbr), nhb = min(16, p.mi_cols - 16 * fbc);
     const int cs = d.coeff_shift;
-    const bool border = fbr == 0 || fbc == 0 || 16 * (fbr + 1) >= p.mi_rows || 16 * (fbc + 1) >= p.mi_cols;
-    uint64_t *out_y = d.mse + ((size_t)fb) * 64;
-    uint64_t *out_c = d.mse + ((size_t)d.nvfb * d.nhfb + fb) * 64;
-    if (tid < 32) { // svt_sb_compute_cdef_list: raster list of the non-skip 8x8 blocks (two blocks per lane, ballots)
-        unsigned int m[2];
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const int b = tid + 32 * h, r = (b >> 3) * 2, c = (b & 7) * 2;
-            const bool on = r < nvb && c < nhb && !d.skip8[(size_t)((16 * fbr + r) >> 1) * d.skip_stride + ((16 * fbc + c) >> 1)];
-            m[h] = __ballot_sync(0xffffffffu, on);
-        }
-#pragma unroll
-        for (int h = 0; h < 2; h++)
-            if ((m[h] >> tid) & 1u) {
-                const int n = (h ? __popc(m[0]) : 0) + __popc(m[h] & ((1u << tid) - 1u));
-                s_by[n] = (uint8_t)((tid + 32 * h) >> 3);
-                s_bx[n] = (uint8_t)(tid & 7);
-            }
-        if (tid == 0) s_count = __popc(m[0]) + __popc(m[1]);
-    }
-    __syncthreads();
-    const int count = s_count;
-    if (count == 0) { // svt_sb_all_skip: not searched; entries defined as 0
-        for (int i = tid; i < 64; i += NT) (chroma_cta ? out_c : out_y)[i] = 0;
+    for (int i = threadIdx.x; i < 64; i += NT) s_mse[i] = 0;
+    const int count = block_list(fb, d.skip8, d.skip_stride, s_by, s_bx);
+    if (count == 0) {
+        store_mse(d, chroma_cta ? 1 : 0, 0, s_mse);
         return;
     }
-    for (int pli = 0; pli < 3; pli++) {
-        if (!chroma_cta && pli) break; // the luma CTA is done after plane 0
-        const int sh = pli ? 1 : 0;
-        const int pw = (p.mi_cols * 4) >> sh, ph = (p.mi_rows * 4) >> sh;
-        const int bh = (nvb * 4) >> sh, bw = (nhb * 4) >> sh;
-        const int y0 = (fbr * 64) >> sh, x0 = (fbc * 64) >> sh;
-        __syncthreads();
-        load_tile<T>(d.recon.p[pli], d.recon.stride[pli], pw, ph, y0, x0, bh, bw, tile);
-        for (int i = tid; i < 64; i += NT) s_mse[i] = 0;
-        __syncthreads();
+    for (int pli = 0; pli < (chroma_cta ? 3 : 1); pli++) {
+        const PlaneRect r = stage_plane<T>(fb, d.recon, pli, tile);
         const int16_t *in = tile + 2 * TS + 2;
         if (pli == 0) {
             find_dirs(in, s_by, s_bx, count, cs, s_dir, s_var);
             __syncthreads();
             if (chroma_cta) continue; // directions only
         }
-        const int damping = p.pri_damping + cs - (pli != 0);
-        if (pli == 0) {
-            if (border)
-                plane_search_grid<T, 8, NSEC, true, true>(d, gd.g, in, count, s_by, s_bx, s_dir, s_var, s_mse, s_sums, pli, y0, x0, damping);
+        const int damping = d.p.pri_damping + cs - (pli != 0);
+        if constexpr (NSEC == 0) {
+            plane_search_list<T>(d, in, count, s_by, s_bx, s_dir, s_var, s_mse, pli, r.y0, r.x0, damping, fb.border);
+        } else if (pli == 0) {
+            if (fb.border)
+                plane_search_grid<T, 8, NSEC, true, true>(d, d.g, in, count, s_by, s_bx, s_dir, s_var, s_mse, s_sums, pli, r.y0, r.x0, damping);
             else
-                plane_search_grid<T, 8, NSEC, true, false>(d, gd.g, in, count, s_by, s_bx, s_dir, s_var, s_mse, s_sums, pli, y0, x0, damping);
+                plane_search_grid<T, 8, NSEC, true, false>(d, d.g, in, count, s_by, s_bx, s_dir, s_var, s_mse, s_sums, pli, r.y0, r.x0, damping);
         } else {
-            if (border)
-                plane_search_grid<T, 4, NSEC, false, true>(d, gd.g, in, count, s_by, s_bx, s_dir, s_var, s_mse, s_sums, pli, y0, x0, damping);
+            if (fb.border)
+                plane_search_grid<T, 4, NSEC, false, true>(d, d.g, in, count, s_by, s_bx, s_dir, s_var, s_mse, s_sums, pli, r.y0, r.x0, damping);
             else
-                plane_search_grid<T, 4, NSEC, false, false>(d, gd.g, in, count, s_by, s_bx, s_dir, s_var, s_mse, s_sums, pli, y0, x0, damping);
+                plane_search_grid<T, 4, NSEC, false, false>(d, d.g, in, count, s_by, s_bx, s_dir, s_var, s_mse, s_sums, pli, r.y0, r.x0, damping);
         }
         __syncthreads();
-        for (int gi = tid; gi < 64; gi += NT) {
-            const unsigned long long v = gi < p.n_strengths ? (s_mse[gi] >> (2 * cs)) : 0;
-            if (pli == 0)
-                out_y[gi] = v;
-            else if (pli == 1)
-                out_c[gi] = v;
-            else
-                out_c[gi] += v;
-        }
+        store_mse(d, pli, count, s_mse);
     }
 }
 
@@ -737,6 +678,12 @@ struct CdefApplyDev {
     int nvfb, nhfb, coeff_shift;
 };
 
+// A signalled strength, pri * 4 + sec with sec 3 standing for 4, as the filter's (pri, sec)
+__device__ __forceinline__ int2 decode_strength(int s) {
+    const int sec = s % 4;
+    return make_int2(s / 4, sec + (sec == 3));
+}
+
 // Tried: one CTA per 32x32 QUADRANT of the filter block (4x the CTAs, a quarter of the serial chain each): bit-exact but
 // slower at 1080p and at 2160p 10-bit: the rim samples and the per-quadrant set-up cost more than the shorter chain saves - the kernel is throughput
 // bound (12 taps x constrain() per sample), not latency bound.  One CTA per filter block kept.
@@ -748,44 +695,32 @@ __global__ void __launch_bounds__(NT) cdef_apply_kernel(const __grid_constant__ 
     __shared__ int s_var[64];
     __shared__ int s_any;
     const int tid = threadIdx.x;
-    const int fb = blockIdx.x, fbr = fb / d.nhfb, fbc = fb - fbr * d.nhfb;
     const SvtB200CdefApplyParams &p = d.p;
-    const int nvb = min(16, p.mi_rows - 16 * fbr), nhb = min(16, p.mi_cols - 16 * fbc);
+    const FilterBlock fb(blockIdx.x, d.nhfb, p.mi_rows, p.mi_cols);
     const int cs = d.coeff_shift;
-    // does the +2 rim of this filter block reach outside the frame (CDEF_VERY_LARGE samples present)?
-    const bool border = fbr == 0 || fbc == 0 || 16 * (fbr + 1) >= p.mi_rows || 16 * (fbc + 1) >= p.mi_cols;
-    const int idx = d.fb_idx[fb];
-    int level = 0, sec = 0, uv_level = 0, uv_sec = 0;
+    const bool border = fb.border; // read once here: read from fb in the sample loop, the kernel takes 8 more registers
+    const int idx = d.fb_idx[blockIdx.x];
+    int2 y = make_int2(0, 0), uv = make_int2(0, 0); // (primary, secondary) strength of luma and of chroma
     if (idx >= 0) {
-        const int ys = d.dec ? d.dec->y_strength[idx] : p.y_strength[idx], uvs = d.dec ? d.dec->uv_strength[idx] : p.uv_strength[idx];
-        level = ys / 4;
-        sec = ys % 4;
-        sec += sec == 3;
-        uv_level = uvs / 4;
-        uv_sec = uvs % 4;
-        uv_sec += uv_sec == 3;
+        y = decode_strength(d.dec ? d.dec->y_strength[idx] : p.y_strength[idx]);
+        uv = decode_strength(d.dec ? d.dec->uv_strength[idx] : p.uv_strength[idx]);
     }
-    const bool fb_on = idx >= 0 && !(level == 0 && sec == 0 && uv_level == 0 && uv_sec == 0);
+    const bool fb_on = idx >= 0 && !(y.x == 0 && y.y == 0 && uv.x == 0 && uv.y == 0);
     if (tid == 0) s_any = 0;
     __syncthreads();
     if (tid < 64) {
         const int by = tid >> 3, bx = tid & 7;
         int sk = 1;
-        if (fb_on && 2 * by < nvb && 2 * bx < nhb)
-            sk = d.skip8[(size_t)((16 * fbr + 2 * by) >> 1) * d.skip_stride + ((16 * fbc + 2 * bx) >> 1)];
+        if (fb_on && 2 * by < fb.nvb && 2 * bx < fb.nhb)
+            sk = d.skip8[(size_t)((16 * fb.fbr + 2 * by) >> 1) * d.skip_stride + ((16 * fb.fbc + 2 * bx) >> 1)];
         s_skip[tid] = (uint8_t)sk;
         if (!sk) s_any = 1;
     }
     __syncthreads();
     const bool filt = fb_on && s_any;
     for (int pli = 0; pli < 3; pli++) {
-        const int sh = pli ? 1 : 0, bs = 8 >> sh;
-        const int pw = (p.mi_cols * 4) >> sh, ph = (p.mi_rows * 4) >> sh;
-        const int bh = (nvb * 4) >> sh, bw = (nhb * 4) >> sh;
-        const int y0 = (fbr * 64) >> sh, x0 = (fbc * 64) >> sh;
-        __syncthreads();
-        load_tile<T>(d.recon.p[pli], d.recon.stride[pli], pw, ph, y0, x0, bh, bw, tile);
-        __syncthreads();
+        const int sh = pli ? 1 : 0;
+        const PlaneRect rect = stage_plane<T>(fb, d.recon, pli, tile);
         const int16_t *in = tile + 2 * TS + 2;
         if (pli == 0 && filt) {
             for (int b0 = 0; b0 < 64; b0 += NT / 8) { // eight lanes per block; skipped blocks are computed and dropped
@@ -799,13 +734,13 @@ __global__ void __launch_bounds__(NT) cdef_apply_kernel(const __grid_constant__ 
             }
             __syncthreads();
         }
-        const int pri = (pli ? uv_level : level) << cs, s2 = (pli ? uv_sec : sec) << cs;
+        const int pri = (pli ? uv.x : y.x) << cs, s2 = (pli ? uv.y : y.y) << cs;
         const int damping = p.damping + cs - (pli != 0);
         T *op = reinterpret_cast<T *>(const_cast<void *>(d.out.p[pli]));
         const int ostride = d.out.stride[pli];
         // four samples of one block row per thread: direction, strengths, tap offsets and shifts are per-block values
-        const int q4 = bw >> 2;
-        for (int i = tid; i < bh * q4; i += NT) {
+        const int q4 = rect.bw >> 2;
+        for (int i = tid; i < rect.bh * q4; i += NT) {
             const int r = i / q4, c = (i - r * q4) << 2;
             const int b = (r >> (3 - sh)) * 8 + (c >> (3 - sh));
             const int16_t *q = in + r * TS + c;
@@ -818,7 +753,7 @@ __global__ void __launch_bounds__(NT) cdef_apply_kernel(const __grid_constant__ 
                     for (int j = 0; j < 4; j++) o[j] = border ? cdef_px<true>(q + j, taps, t, s2) : cdef_px<false>(q + j, taps, t, s2);
                 }
             }
-            T *dst = op + (size_t)(y0 + r) * ostride + x0 + c;
+            T *dst = op + (size_t)(rect.y0 + r) * ostride + rect.x0 + c;
             if (sizeof(T) == 1 && ((uintptr_t)dst & 3) == 0)
                 *reinterpret_cast<uint32_t *>(dst) = (uint32_t)o[0] | ((uint32_t)o[1] << 8) | ((uint32_t)o[2] << 16) | ((uint32_t)o[3] << 24);
             else if (sizeof(T) == 2 && ((uintptr_t)dst & 7) == 0)
@@ -850,7 +785,10 @@ __global__ void filter_block_kernel(const uint16_t *win, int pri, int sec, int d
     for (int i = threadIdx.x; i < 144; i += blockDim.x) t[i] = (int16_t)win[i];
     __syncthreads();
     const int i = threadIdx.x >> 3, j = threadIdx.x & 7;
-    if (i < rows && j < cols) out[i * 8 + j] = (uint16_t)cdef_sample(t + (i + 2) * 12 + j + 2, 12, pri, sec, dir, pd, sd, coeff_shift);
+    if (i < rows && j < cols) {
+        const CdefTaps taps = make_taps(pri, sec, dir, pd, sd, coeff_shift, 12);
+        out[i * 8 + j] = (uint16_t)cdef_px<true>(t + (i + 2) * 12 + j + 2, taps, pri, sec);
+    }
 }
 
 static int frame_dev(const SvtB200Frame *f, FrameDev *o) {
@@ -1076,6 +1014,56 @@ __global__ void __launch_bounds__(1024) cdef_decide_kernel(const DecideDev d) {
     }
 }
 
+// Every table of get_cdef_filter_strengths is a grid, gi = pi * nsec + si with nsec 2 or 4 and at most 16 primary
+// strengths: returns nsec and fills g, or 0 for any other strength list (g zeroed).
+static int strength_grid(const SvtB200CdefSearchParams &p, CdefGrid &g) {
+    memset(&g, 0, sizeof(g));
+    int nsec = 1;
+    while (nsec < p.n_strengths && p.pri_strength[nsec] == p.pri_strength[0]) nsec++;
+    bool grid = (nsec == 2 || nsec == 4) && p.n_strengths % nsec == 0 && p.n_strengths / nsec <= 16;
+    for (int gi = 0; grid && gi < p.n_strengths; gi++)
+        grid = p.pri_strength[gi] == p.pri_strength[gi / nsec * nsec] && p.sec_strength[gi] == p.sec_strength[gi % nsec];
+    if (!grid) return 0;
+    g.npri = p.n_strengths / nsec;
+    for (int i = 0; i < g.npri; i++) g.pri[i] = p.pri_strength[i * nsec];
+    for (int i = 0; i < nsec; i++) g.sec[i] = p.sec_strength[i];
+    return nsec;
+}
+template <typename T>
+static void launch_search(int nsec, const CdefSearchDev &d, cudaStream_t st) {
+    const dim3 grid(d.nvfb * d.nhfb, 2);
+    if (nsec == 4)
+        SVTB_LAUNCH((cdef_search_kernel<T, 4>), grid, NT, 0, st, d);
+    else if (nsec == 2)
+        SVTB_LAUNCH((cdef_search_kernel<T, 2>), grid, NT, 0, st, d);
+    else
+        SVTB_LAUNCH((cdef_search_kernel<T, 0>), grid, NT, 0, st, d);
+}
+
+// The two apply entries once d holds the strengths (host params, or the device decision): the argument checks, the
+// filter-block grid and the launch.  `strengths` is false when the entry was given none.
+static int apply_launch(const char *entry, CdefApplyDev &d, bool strengths, const SvtB200Frame *recon, const SvtB200Frame *out,
+                        const uint8_t *skip8, int32_t skip_stride, const int8_t *fb_strength_idx, void *stream) {
+    if (!strengths || !skip8 || !fb_strength_idx || frame_dev(recon, &d.recon) || frame_dev(out, &d.out) ||
+        recon->bit_depth != out->bit_depth || recon->y == out->y) {
+        set_error("%s: bad argument (out must not alias recon)", entry);
+        return SVT_B200_ERR_ARG;
+    }
+    d.skip8 = skip8;
+    d.skip_stride = skip_stride;
+    d.fb_idx = fb_strength_idx;
+    d.nvfb = fb_count(d.p.mi_rows);
+    d.nhfb = fb_count(d.p.mi_cols);
+    d.coeff_shift = recon->bit_depth - 8;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (d.recon.hbd)
+        SVTB_LAUNCH(cdef_apply_kernel<uint16_t>, d.nvfb * d.nhfb, NT, 0, st, d);
+    else
+        SVTB_LAUNCH(cdef_apply_kernel<uint8_t>, d.nvfb * d.nhfb, NT, 0, st, d);
+    SVTB_CUDA_TRY(cudaGetLastError());
+    return SVT_B200_OK;
+}
+
 extern "C" {
 
 int svt_b200_cdef_strength_table(int pick_method, SvtB200CdefSearchParams *p) {
@@ -1107,67 +1095,23 @@ int svt_b200_cdef_search(const SvtB200CdefSearchParams *p, const SvtB200Frame *r
     d.skip8 = skip8;
     d.skip_stride = skip_stride;
     d.mse = mse;
-    d.nvfb = (p->mi_rows + 15) / 16;
-    d.nhfb = (p->mi_cols + 15) / 16;
+    d.nvfb = fb_count(p->mi_rows);
+    d.nhfb = fb_count(p->mi_cols);
     d.coeff_shift = recon->bit_depth - 8;
-    cudaStream_t st = (cudaStream_t)stream;
-    // grid-structured table (every table of get_cdef_filter_strengths is one): separable kernel
-    CdefSearchGridDev gd;
-    int nsec = 1;
-    while (nsec < p->n_strengths && p->pri_strength[nsec] == p->pri_strength[0]) nsec++;
-    bool grid = (nsec == 2 || nsec == 4) && p->n_strengths % nsec == 0 && p->n_strengths / nsec <= 16;
-    for (int gi = 0; grid && gi < p->n_strengths; gi++)
-        grid = p->pri_strength[gi] == p->pri_strength[gi / nsec * nsec] && p->sec_strength[gi] == p->sec_strength[gi % nsec];
-    if (grid) {
-        gd.d = d;
-        gd.g.npri = p->n_strengths / nsec;
-        gd.g.nsec = nsec;
-        memset(gd.g.pri, 0, sizeof(gd.g.pri));
-        memset(gd.g.sec, 0, sizeof(gd.g.sec));
-        for (int i = 0; i < gd.g.npri; i++) gd.g.pri[i] = p->pri_strength[i * nsec];
-        for (int i = 0; i < nsec; i++) gd.g.sec[i] = p->sec_strength[i];
-        if (d.recon.hbd) {
-            if (nsec == 2)
-                SVTB_LAUNCH((cdef_search_grid_kernel<uint16_t, 2>), dim3(d.nvfb * d.nhfb, 2), NT, 0, st, gd);
-            else
-                SVTB_LAUNCH((cdef_search_grid_kernel<uint16_t, 4>), dim3(d.nvfb * d.nhfb, 2), NT, 0, st, gd);
-        } else {
-            if (nsec == 2)
-                SVTB_LAUNCH((cdef_search_grid_kernel<uint8_t, 2>), dim3(d.nvfb * d.nhfb, 2), NT, 0, st, gd);
-            else
-                SVTB_LAUNCH((cdef_search_grid_kernel<uint8_t, 4>), dim3(d.nvfb * d.nhfb, 2), NT, 0, st, gd);
-        }
-    } else if (d.recon.hbd)
-        SVTB_LAUNCH(cdef_search_kernel<uint16_t>, d.nvfb * d.nhfb, NT, 0, st, d);
+    const int nsec = strength_grid(*p, d.g);
+    if (d.recon.hbd)
+        launch_search<uint16_t>(nsec, d, (cudaStream_t)stream);
     else
-        SVTB_LAUNCH(cdef_search_kernel<uint8_t>, d.nvfb * d.nhfb, NT, 0, st, d);
+        launch_search<uint8_t>(nsec, d, (cudaStream_t)stream);
     SVTB_CUDA_TRY(cudaGetLastError());
     return SVT_B200_OK;
 }
 
 int svt_b200_cdef_apply(const SvtB200CdefApplyParams *p, const SvtB200Frame *recon, const SvtB200Frame *out,
                         const uint8_t *skip8, int32_t skip_stride, const int8_t *fb_strength_idx, void *stream) {
-    CdefApplyDev d;
-    if (!p || !skip8 || !fb_strength_idx || frame_dev(recon, &d.recon) || frame_dev(out, &d.out) ||
-        recon->bit_depth != out->bit_depth || recon->y == out->y) {
-        set_error("svt_b200_cdef_apply: bad argument (out must not alias recon)");
-        return SVT_B200_ERR_ARG;
-    }
-    d.p = *p;
-    d.dec = nullptr;
-    d.skip8 = skip8;
-    d.skip_stride = skip_stride;
-    d.fb_idx = fb_strength_idx;
-    d.nvfb = (p->mi_rows + 15) / 16;
-    d.nhfb = (p->mi_cols + 15) / 16;
-    d.coeff_shift = recon->bit_depth - 8;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (d.recon.hbd)
-        SVTB_LAUNCH(cdef_apply_kernel<uint16_t>, d.nvfb * d.nhfb, NT, 0, st, d);
-    else
-        SVTB_LAUNCH(cdef_apply_kernel<uint8_t>, d.nvfb * d.nhfb, NT, 0, st, d);
-    SVTB_CUDA_TRY(cudaGetLastError());
-    return SVT_B200_OK;
+    CdefApplyDev d{};
+    if (p) d.p = *p;
+    return apply_launch("svt_b200_cdef_apply", d, p != nullptr, recon, out, skip8, skip_stride, fb_strength_idx, stream);
 }
 
 int svt_b200_cdef_decide_table(int pick_method, SvtB200CdefDecideParams *p) {
@@ -1193,8 +1137,8 @@ int svt_b200_cdef_decide(const SvtB200CdefDecideParams *p, const uint64_t *mse, 
     }
     DecideDev d;
     d.p = *p;
-    d.nvfb = (p->mi_rows + 15) / 16;
-    d.nhfb = (p->mi_cols + 15) / 16;
+    d.nvfb = fb_count(p->mi_rows);
+    d.nhfb = fb_count(p->mi_cols);
     const size_t nfb = (size_t)d.nvfb * d.nhfb;
     d.mse0 = reinterpret_cast<const unsigned long long *>(mse);
     d.mse1 = d.mse0 + nfb * 64;
@@ -1216,28 +1160,10 @@ int svt_b200_cdef_decide(const SvtB200CdefDecideParams *p, const uint64_t *mse, 
 int svt_b200_cdef_apply_dev(int32_t mi_rows, int32_t mi_cols, int32_t damping, const SvtB200CdefDecision *decision,
                             const SvtB200Frame *recon, const SvtB200Frame *out, const uint8_t *skip8, int32_t skip_stride,
                             const int8_t *fb_strength_idx, void *stream) {
-    CdefApplyDev d;
-    if (!decision || !skip8 || !fb_strength_idx || frame_dev(recon, &d.recon) || frame_dev(out, &d.out) ||
-        recon->bit_depth != out->bit_depth || recon->y == out->y) {
-        set_error("svt_b200_cdef_apply_dev: bad argument (out must not alias recon)");
-        return SVT_B200_ERR_ARG;
-    }
-    memset(&d.p, 0, sizeof(d.p));
+    CdefApplyDev d{};
     d.p.mi_rows = mi_rows, d.p.mi_cols = mi_cols, d.p.damping = damping;
     d.dec = decision;
-    d.skip8 = skip8;
-    d.skip_stride = skip_stride;
-    d.fb_idx = fb_strength_idx;
-    d.nvfb = (mi_rows + 15) / 16;
-    d.nhfb = (mi_cols + 15) / 16;
-    d.coeff_shift = recon->bit_depth - 8;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (d.recon.hbd)
-        SVTB_LAUNCH(cdef_apply_kernel<uint16_t>, d.nvfb * d.nhfb, NT, 0, st, d);
-    else
-        SVTB_LAUNCH(cdef_apply_kernel<uint8_t>, d.nvfb * d.nhfb, NT, 0, st, d);
-    SVTB_CUDA_TRY(cudaGetLastError());
-    return SVT_B200_OK;
+    return apply_launch("svt_b200_cdef_apply_dev", d, decision != nullptr, recon, out, skip8, skip_stride, fb_strength_idx, stream);
 }
 
 int32_t svt_cdef_find_dir_cuda(const uint16_t *img, int32_t stride, int32_t *var, int32_t coeff_shift) {

@@ -65,9 +65,9 @@ def test_cdef_search_vs_oracle(case):
     np.testing.assert_array_equal(got, want)
 
 
-@pytest.mark.parametrize("case", [(192, 136, 8), (200, 72, 10)])
+@pytest.mark.parametrize("case", [(192, 136, 8), (200, 72, 10), (640, 360, 10)])
 def test_cdef_search_arbitrary_table(case):
-    """A strength list that is NOT a pri x sec grid takes the generic (one pass per strength) kernel."""
+    """A strength list that is NOT a pri x sec grid takes the list form of the search kernel (one pass per strength)."""
     import gpu_runner as gr
     w, h, bd = case
     src, rec, mi_rows, mi_cols, skip = cdef_picture_case(w, h, bd, seed=5)
