@@ -9,12 +9,17 @@
 //   svt_av1_quantize_fp[_32x32/_64x64], svt_av1_highbd_quantize_fp  Encoder/Codec/EbFullLoop.c:314-600
 //   the per-TU body of av1_encode_loop (EbCodingLoop.c:290-...) as ONE fused kernel:
 //       residual -> forward txfm -> quantise/dequantise -> inverse txfm -> reconstruct
+//   open_loop_intra_search_mb of the TPL path (DC_PRED, 16x16 DCT cost) for a whole picture
 //
 // Design: a transform block lives in shared memory for its whole life (w x h int32, odd pitch); one thread
 // owns a column in the column pass and a row in the row pass, so a 64x64 block is 64 lanes and small blocks
-// are packed several per CTA.  In the fused kernel HBM sees only src + pred in and qcoeff + recon out
-// (7 B/px for 8-bit, SURVEY §8d) — the int32 coefficient planes of the reference's five separate calls never
-// leave the SM.
+// are packed several per CTA.  The 2-D transforms are written once, fwd_txfm2d and inv_txfm2d (txfm.cuh), and every
+// kernel runs them: the forward and inverse drop-ins (one block), the fused kernel (specialised per square size
+// through make_txcfg<TS>) and the open-loop intra search (16x16 DCT).  In the fused kernel HBM sees only src + pred in
+// and qcoeff + recon out (7 B/px for 8-bit, SURVEY §8d) — the int32 coefficient planes of the reference's five
+// separate calls never leave the SM.
+//
+// Layout: tables and kernels, then the host helpers, then every exported entry in one extern "C" block.
 #include <algorithm>
 #include <vector>
 
@@ -26,21 +31,56 @@
 
 namespace svtb200 {
 
-__constant__ uint8_t c_txw[19] = {4, 8, 16, 32, 64, 4, 8, 8, 16, 16, 32, 32, 64, 4, 16, 8, 32, 16, 64};
-__constant__ uint8_t c_txh[19] = {4, 8, 16, 32, 64, 8, 4, 16, 8, 32, 16, 64, 32, 16, 4, 32, 8, 64, 16};
+// Width and height per TxSize (TX_4X4 .. TX_64X16) and the 1-D kinds of the columns (vtx) and rows (htx) per TxType
+// (0 DCT, 1 ADST, 2 FLIPADST, 3 IDTX).  The host reads these; tx_setup() uploads them to the __constant__ copies below
+// for the kernels, and a kernel specialised for one size reads them at compile time (tx_w_dev).
+constexpr uint8_t k_txw[19] = {4, 8, 16, 32, 64, 4, 8, 8, 16, 16, 32, 32, 64, 4, 16, 8, 32, 16, 64};
+constexpr uint8_t k_txh[19] = {4, 8, 16, 32, 64, 8, 4, 16, 8, 32, 16, 64, 32, 16, 4, 32, 8, 64, 16};
+constexpr uint8_t k_vtx[16] = {0, 1, 0, 1, 2, 0, 2, 1, 2, 3, 0, 3, 1, 3, 2, 3};
+constexpr uint8_t k_htx[16] = {0, 0, 1, 1, 0, 2, 2, 2, 1, 3, 3, 0, 3, 1, 3, 2};
+// the coded part of a side: 64-wide transforms keep their top-left 32 x 32 coefficients
+__host__ __device__ constexpr int tx_coded(int n) { return n < 32 ? n : 32; }
+// scan of a transform type (get_scan): 1 row scan for V_* (identity rows), 2 column scan for H_*, 0 the default scan
+__host__ __device__ constexpr int scan_class(int vk, int hk) { return (vk != 3 && hk == 3) ? 1 : (vk == 3 && hk != 3) ? 2 : 0; }
+
+__constant__ uint8_t c_txw[19];
+__constant__ uint8_t c_txh[19];
 __constant__ int8_t c_fwd_shift[19][3] = {{2, 0, 0},  {2, -1, 0}, {2, -2, 0}, {2, -4, 0}, {0, -2, -2}, {2, -1, 0}, {2, -1, 0},
                                           {2, -2, 0}, {2, -2, 0}, {2, -4, 0}, {2, -4, 0}, {0, -2, -2}, {2, -4, -2}, {2, -1, 0},
                                           {2, -1, 0}, {2, -2, 0}, {2, -2, 0}, {0, -2, 0}, {2, -4, 0}};
 __constant__ int8_t c_inv_shift0[19] = {0, -1, -2, -2, -2, 0, 0, -1, -1, -1, -1, -1, -1, -1, -1, -2, -2, -2, -2};
 __constant__ int8_t c_fwd_cos_col[5][5] = {{13, 13, 13, 0, 0}, {13, 13, 13, 12, 0}, {13, 13, 13, 12, 13}, {0, 13, 13, 12, 13}, {0, 0, 13, 12, 13}};
 __constant__ int8_t c_fwd_cos_row[5][5] = {{13, 13, 12, 0, 0}, {13, 13, 13, 12, 0}, {13, 13, 12, 13, 12}, {0, 12, 13, 12, 11}, {0, 0, 12, 11, 10}};
-__constant__ uint8_t c_vtx[16] = {0, 1, 0, 1, 2, 0, 2, 1, 2, 3, 0, 3, 1, 3, 2, 3};
-__constant__ uint8_t c_htx[16] = {0, 0, 1, 1, 0, 2, 2, 2, 1, 3, 3, 0, 3, 1, 3, 2};
+__constant__ uint8_t c_vtx[16];
+__constant__ uint8_t c_htx[16];
 
-static const uint8_t h_txw[19] = {4, 8, 16, 32, 64, 4, 8, 8, 16, 16, 32, 32, 64, 4, 16, 8, 32, 16, 64};
-static const uint8_t h_txh[19] = {4, 8, 16, 32, 64, 8, 4, 16, 8, 32, 16, 64, 32, 16, 4, 32, 8, 64, 16};
+// Width / height of a transform in device code: a compile-time constant in a kernel specialised for size TS >= 0, so
+// that its loop bounds and 1-D sizes fold; the __constant__ table for TS = -1 (any size).
+template <int TS>
+__device__ __forceinline__ int tx_w_dev(int tx_size) {
+    if constexpr (TS >= 0) {
+        constexpr int w = k_txw[TS];
+        return w;
+    } else {
+        return c_txw[tx_size];
+    }
+}
+template <int TS>
+__device__ __forceinline__ int tx_h_dev(int tx_size) {
+    if constexpr (TS >= 0) {
+        constexpr int h = k_txh[TS];
+        return h;
+    } else {
+        return c_txh[tx_size];
+    }
+}
 
+// av1_transform_config / svt_av1_get_inv_txfm_cfg of (tx_size, tx_type).  TS >= 0 fixes the size: the fields derived
+// from it are read from the tables as for any size, then w and h become compile-time constants, so that the passes
+// over t (fwd_txfm2d, inv_txfm2d) get compile-time loop bounds and 1-D sizes.
+template <int TS = -1>
 __device__ TxCfg make_txcfg(int tx_size, int tx_type) {
+    if (TS >= 0) tx_size = TS;
     TxCfg t;
     t.w = c_txw[tx_size];
     t.h = c_txh[tx_size];
@@ -57,6 +97,8 @@ __device__ TxCfg make_txcfg(int tx_size, int tx_type) {
     t.cbc = c_fwd_cos_col[wi][hi];
     t.cbr = c_fwd_cos_row[wi][hi];
     t.rect = (t.w == 2 * t.h) || (t.h == 2 * t.w);
+    t.w = tx_w_dev<TS>(tx_size);
+    t.h = tx_h_dev<TS>(tx_size);
     return t;
 }
 
@@ -67,7 +109,9 @@ using namespace svtb200;
 namespace {
 
 constexpr int TX_NT = 128; // threads per CTA of the transform kernels
-__host__ __device__ inline int tx_pitch(int w) { return w | 1; } // odd pitch: conflict-free row pass
+__host__ __device__ constexpr int tx_pitch(int w) { return w | 1; } // odd pitch: conflict-free row pass
+// blocks of a w x h transform per CTA: one lane per column / row of the longer side
+__host__ __device__ constexpr int tx_bpc(int w, int h) { return TX_NT / (w > h ? w : h); }
 
 // One descriptor per transform unit of a batched launch.
 struct TuDev {
@@ -77,145 +121,65 @@ struct TuDev {
 };
 
 // ---------------------------------------------------------------------------------------------------------------
-// forward: residual (int16, strided) -> coefficients (int32, contiguous w x h; 64-wide sizes optionally re-packed)
+// forward drop-in: one residual block (int16, w x h) -> coefficients (int32, contiguous w x h)
 // ---------------------------------------------------------------------------------------------------------------
 struct FwdArgs {
-    const int16_t *in; // block b at in + b * in_block_stride
-    size_t in_block_stride;
-    int in_stride;
-    int32_t *out; // block b at out + b * w*h
-    const int32_t *tx_types; // per block (device) or null -> tx_type
-    int tx_type, tx_size, n_blocks;
+    const int16_t *in;
+    int32_t *out;
+    int tx_type, tx_size;
     int pf_shift; // 0 full, 1 N2, 2 N4: keep only the top-left (w>>s) x (h>>s) coefficients (EbTransforms.c:5401,7007)
-    int repack64; // 1: svt_handle_transform* semantics (zero the dropped area, pack 32-wide, energy -> energy[b])
-    uint64_t *energy;
 };
 __global__ void __launch_bounds__(TX_NT) fwd_txfm_kernel(const FwdArgs a) {
     extern __shared__ int32_t sm[];
-    const int w = c_txw[a.tx_size], h = c_txh[a.tx_size];
-    const int T = max(w, h), bpc = TX_NT / T, pitch = tx_pitch(w);
-    const int lb = threadIdx.x / T, li = threadIdx.x % T;
-    const int b = blockIdx.x * bpc + lb;
-    const bool live = b < a.n_blocks && lb < bpc;
-    int32_t *buf = sm + lb * (pitch * h);
-    TxCfg t = make_txcfg(a.tx_size, live && a.tx_types ? a.tx_types[b] : a.tx_type);
-    if (live) {
-        const int16_t *src = a.in + (size_t)b * a.in_block_stride;
+    const TxCfg t = make_txcfg(a.tx_size, a.tx_type);
+    const int w = t.w, h = t.h, T = max(w, h), pitch = tx_pitch(w), li = threadIdx.x;
+    const bool live = li < T; // one block: the lanes past its longer side idle
+    if (live)
         for (int i = li; i < w * h; i += T) {
             const int r = i / w, c = i - r * w;
-            buf[r * pitch + c] = src[(size_t)(t.ud ? h - 1 - r : r) * a.in_stride + (t.lr ? w - 1 - c : c)];
+            sm[r * pitch + c] = a.in[(t.ud ? h - 1 - r : r) * w + (t.lr ? w - 1 - c : c)];
         }
-    }
+    __syncthreads();
+    fwd_txfm2d(sm, pitch, t, li, T, live);
     __syncthreads();
     if (live) {
-        for (int c = li; c < t.w; c += T) { /* column pass */
-            const int fs0 = t.fs0, fs1 = t.fs1;
-            fwd_1d_pass(buf + c, pitch, t.h, t.vk, t.cbc, [=](int32_t v) { return (int32_t)((uint32_t)v << fs0); },
-                        [=](int32_t v) { return fs1 ? round_shift64((long long)v, -fs1) : v; });
-        }
-    }
-    __syncthreads();
-    if (live) {
-        for (int r = li; r < t.h; r += T) { /* row pass */
-            const int fs2 = t.fs2, rect = t.rect;
-            fwd_1d_pass(buf + r * pitch, 1, t.w, t.hk, t.cbr, [](int32_t v) { return v; }, [=](int32_t v) {
-                if (fs2) v = round_shift64((long long)v, -fs2);
-                if (rect) v = round_shift64((long long)v * 5793, 12);
-                return v;
-            });
-        }
-    }
-    __syncthreads();
-    __shared__ unsigned long long s_e2[TX_NT];
-    unsigned long long e = 0;
-    if (live) {
-        int32_t *dst = a.out + (size_t)b * w * h;
-        if (!a.repack64) {
-            const int kw2 = w >> a.pf_shift, kh2 = h >> a.pf_shift;
-            for (int i = li; i < w * h; i += T) dst[i] = ((i % w) < kw2 && (i / w) < kh2) ? buf[(i / w) * pitch + (i % w)] : 0;
-        } else {
-            // svt_handle_transform* (EbTransforms.c:2763-2931): energy of the dropped area, zero it, then re-pack the
-            // kept 32-wide rows to the front.  Entries behind the packed block keep what the in-place C code leaves.
-            const int kw = min(w, 32), kh = min(h, 32);
-            for (int i = li; i < w * h; i += T) {
-                const int r = i / w, c = i - r * w;
-                const int32_t v = buf[r * pitch + c];
-                const bool dropped = r >= kh || c >= kw;
-                if (dropped) e += (unsigned long long)((long long)v * (long long)v);
-                dst[i] = (kw != w && i < kw * kh) ? buf[(i / kw) * pitch + (i % kw)] : (dropped ? 0 : v);
-            }
-        }
-    }
-    if (a.repack64) { // uniform branch: CTA-wide barrier is safe
-        s_e2[threadIdx.x] = e;
-        __syncthreads();
-        if (live && li == 0 && a.energy) {
-            unsigned long long tot = 0;
-            for (int i = 0; i < T; i++) tot += s_e2[lb * T + i];
-            a.energy[b] = tot;
-        }
+        const int kw = w >> a.pf_shift, kh = h >> a.pf_shift;
+        for (int i = li; i < w * h; i += T) a.out[i] = ((i % w) < kw && (i / w) < kh) ? sm[(i / w) * pitch + (i % w)] : 0;
     }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// inverse: coefficients -> residual added to the prediction, clipped (svt_av1_inv_txfm2d_add_*)
+// inverse drop-in: one block of coefficients (64-wide sizes: the 32-wide packed input) -> residual added to the
+// prediction, clipped (svt_av1_inv_txfm2d_add_*); prediction and reconstruction are w x h
 // ---------------------------------------------------------------------------------------------------------------
 struct InvArgs {
-    const int32_t *in; // block b at in + b * iw*ih (64-wide sizes: 32-wide packed input)
+    const int32_t *in;
     const uint16_t *pred;
-    uint16_t *recon; // block b at + b * block_stride
-    size_t pred_block_stride, recon_block_stride;
-    int stride_r, stride_w;
-    int tx_type, tx_size, n_blocks, bd;
+    uint16_t *recon;
+    int tx_type, tx_size, bd;
 };
 __global__ void __launch_bounds__(TX_NT) inv_txfm_kernel(const InvArgs a) {
     extern __shared__ int32_t sm[];
-    const int w = c_txw[a.tx_size], h = c_txh[a.tx_size];
-    const int iw = min(w, 32), ih = min(h, 32);
-    const int T = max(w, h), bpc = TX_NT / T, pitch = tx_pitch(w);
-    const int lb = threadIdx.x / T, li = threadIdx.x % T;
-    const int b = blockIdx.x * bpc + lb;
-    const bool live = b < a.n_blocks && lb < bpc;
-    int32_t *buf = sm + lb * (pitch * h);
-    TxCfg t = make_txcfg(a.tx_size, a.tx_type);
-    if (live) {
-        const int32_t *src = a.in + (size_t)b * iw * ih;
+    const TxCfg t = make_txcfg(a.tx_size, a.tx_type);
+    const int w = t.w, h = t.h, iw = tx_coded(w), ih = tx_coded(h);
+    const int T = max(w, h), pitch = tx_pitch(w), li = threadIdx.x;
+    const bool live = li < T; // one block: the lanes past its longer side idle
+    if (live)
         for (int i = li; i < w * h; i += T) {
             const int r = i / w, c = i - r * w;
-            buf[r * pitch + c] = (r < ih && c < iw) ? src[r * iw + c] : 0;
+            sm[r * pitch + c] = (r < ih && c < iw) ? a.in[r * iw + c] : 0;
         }
-    }
     __syncthreads();
-    const int bd = a.bd;
-    const int range_row = bd == 8 ? 16 : bd == 10 ? 18 : 20, range_col = bd == 8 ? 16 : bd == 10 ? 16 : 18;
-    if (live) {
-        for (int r = li; r < t.h; r += T) {
-            const int rect = t.rect, is0 = t.is0;
-            inv_1d_pass(buf + r * pitch, 1, t.w, t.hk, 12, range_row, [=](int32_t v) {
-                if (rect) v = round_shift64((long long)v * 2896, 12);
-                return clampv(v, bd + 8);
-            }, [=](int32_t v) { return is0 ? round_shift64((long long)v, -is0) : v; });
-        }
-    }
+    inv_txfm2d(sm, pitch, t, a.bd, li, T, live, [] {});
     __syncthreads();
     if (live) {
-        const int col_clamp = max(bd + 6, 16);
-        for (int c = li; c < t.w; c += T) {
-            inv_1d_pass(buf + c, pitch, t.h, t.vk, 12, range_col, [=](int32_t v) { return clampv(v, col_clamp); },
-                        [](int32_t v) { return round_shift64((long long)v, 4); });
-        }
-    }
-    __syncthreads();
-    if (live) {
-        const uint16_t *pr = a.pred + (size_t)b * a.pred_block_stride;
-        uint16_t *rc = a.recon + (size_t)b * a.recon_block_stride;
-        const int mx = (1 << bd) - 1;
+        const int mx = (1 << a.bd) - 1;
         for (int i = li; i < w * h; i += T) {
             const int r = i / w, c = i - r * w;
             // lr flip: output column c is the transform of buffer column w-1-c; ud flip: output row r = result row h-1-r
-            const int32_t res = buf[(t.ud ? h - 1 - r : r) * pitch + (t.lr ? w - 1 - c : c)];
-            const long long v = (long long)pr[(size_t)r * a.stride_r + c] + res;
-            rc[(size_t)r * a.stride_w + c] = (uint16_t)(v < 0 ? 0 : (v > mx ? mx : v));
+            const int32_t res = sm[(t.ud ? h - 1 - r : r) * pitch + (t.lr ? w - 1 - c : c)];
+            const long long v = (long long)a.pred[i] + res;
+            a.recon[i] = (uint16_t)(v < 0 ? 0 : (v > mx ? mx : v));
         }
     }
 }
@@ -366,10 +330,10 @@ __device__ __forceinline__ void store4(T *p, const int (&v)[4]) {
 template <typename T, int TS>
 __global__ void __launch_bounds__(TX_NT) encode_tu_kernel(const __grid_constant__ EncodeDev d) {
     extern __shared__ int32_t sm[];
-    const int w = TS >= 0 ? (4 << TS) : c_txw[d.tx_size], h = TS >= 0 ? (4 << TS) : c_txh[d.tx_size];
-    const int iw = min(w, 32), ih = min(h, 32), n = iw * ih;
+    const int w = tx_w_dev<TS>(d.tx_size), h = tx_h_dev<TS>(d.tx_size);
+    const int iw = tx_coded(w), ih = tx_coded(h), n = iw * ih;
     const int lw = 31 - __clz(w), liw = 31 - __clz(iw);
-    const int Tn = max(w, h), bpc = TX_NT / Tn, pitch = tx_pitch(w);
+    const int Tn = max(w, h), bpc = tx_bpc(w, h), pitch = tx_pitch(w);
     const int lb = threadIdx.x / Tn, li = threadIdx.x % Tn;
     const int b = blockIdx.x * bpc + lb;
     const bool live = b < d.n_tus && lb < bpc;
@@ -377,8 +341,7 @@ __global__ void __launch_bounds__(TX_NT) encode_tu_kernel(const __grid_constant_
     __shared__ int s_eob[TX_NT / 4], s_cul[TX_NT / 4];
     TuDev tu = {0, 0, 0, 0};
     if (live) tu = d.tus[b];
-    TxCfg t = make_txcfg(TS >= 0 ? TS : d.tx_size, tu.tx_type);
-    if (TS >= 0) t.w = t.h = 4 << TS;
+    const TxCfg t = make_txcfg<TS>(d.tx_size, tu.tx_type);
     const int pl = tu.plane;
     int dc_sign = 0; // set_dc_sign: 1 negative, 2 positive DC level (held by the thread that quantises position 0)
     if (live) { // residual, four samples per step
@@ -396,22 +359,7 @@ __global__ void __launch_bounds__(TX_NT) encode_tu_kernel(const __grid_constant_
         if (li == 0) s_eob[lb] = s_cul[lb] = 0;
     }
     __syncthreads();
-    if (live)
-        for (int c = li; c < t.w; c += Tn) {
-            const int fs0 = t.fs0, fs1 = t.fs1;
-            fwd_1d_pass(buf + c, pitch, t.h, t.vk, t.cbc, [=](int32_t v) { return (int32_t)((uint32_t)v << fs0); },
-                        [=](int32_t v) { return fs1 ? round_shift64((long long)v, -fs1) : v; });
-        }
-    __syncthreads();
-    if (live)
-        for (int r = li; r < t.h; r += Tn) {
-            const int fs2 = t.fs2, rect = t.rect;
-            fwd_1d_pass(buf + r * pitch, 1, t.w, t.hk, t.cbr, [](int32_t v) { return v; }, [=](int32_t v) {
-                if (fs2) v = round_shift64((long long)v, -fs2);
-                if (rect) v = round_shift64((long long)v * 5793, 12);
-                return v;
-            });
-        }
+    fwd_txfm2d(buf, pitch, t, li, Tn, live);
     __syncthreads();
     // quantise + dequantise in place, in raster order (every coefficient is quantised independently; the scan order
     // only defines eob = 1 + the largest scan index of a non-zero level, looked up for the non-zero levels only).
@@ -419,7 +367,7 @@ __global__ void __launch_bounds__(TX_NT) encode_tu_kernel(const __grid_constant_
     if (live) {
         const int log_scale = (w * h > 256) + (w * h > 1024); // av1_get_tx_scale
         const int mode = d.quant_mode + (d.hbd ? 1 : 0);
-        const int16_t *iscan = d.iscan[(t.vk != 3 && t.hk == 3) ? 1 : (t.vk == 3 && t.hk != 3) ? 2 : 0];
+        const int16_t *iscan = d.iscan[scan_class(t.vk, t.hk)];
         int32_t *qout = d.qoff ? d.qcoeff + d.qoff[b] : d.qcoeff + (size_t)b * n;
         // partial-frequency shapes: the N2 / N4 transforms produce the top-left half / quarter (per dimension) of the
         // default transform's coefficients and zeros elsewhere; ONLY_DC keeps coefficient 0 alone
@@ -450,29 +398,14 @@ __global__ void __launch_bounds__(TX_NT) encode_tu_kernel(const __grid_constant_
     }
     __syncthreads();
     const int bd = d.bd;
-    const int range_row = bd == 8 ? 16 : bd == 10 ? 18 : 20, range_col = bd == 8 ? 16 : bd == 10 ? 16 : 18;
-    if (live) {
+    // the unit's eob and cul_level (complete in s_eob / s_cul after the barrier), published by its first lane
+    inv_txfm2d(buf, pitch, t, bd, li, Tn, live, [=, &d] {
         if (li == 0) {
             const int ob = d.out_idx ? d.out_idx[b] : b;
             d.eob[ob] = (uint16_t)s_eob[lb];
             if (d.cul_level) d.cul_level[ob] = min(63, s_cul[lb]) + (dc_sign == 1 ? 64 : dc_sign == 2 ? 128 : 0);
         }
-        for (int r = li; r < t.h; r += Tn) {
-            const int rect = t.rect, is0 = t.is0;
-            inv_1d_pass(buf + r * pitch, 1, t.w, t.hk, 12, range_row, [=](int32_t v) {
-                if (rect) v = round_shift64((long long)v * 2896, 12);
-                return clampv(v, bd + 8);
-            }, [=](int32_t v) { return is0 ? round_shift64((long long)v, -is0) : v; });
-        }
-    }
-    __syncthreads();
-    if (live) {
-        const int col_clamp = max(bd + 6, 16);
-        for (int c = li; c < t.w; c += Tn) {
-            inv_1d_pass(buf + c, pitch, t.h, t.vk, 12, range_col, [=](int32_t v) { return clampv(v, col_clamp); },
-                        [](int32_t v) { return round_shift64((long long)v, 4); });
-        }
-    }
+    });
     __syncthreads();
     if (live) { // reconstruction, four samples per step
         const T *pp = reinterpret_cast<const T *>(d.pred[pl]) + (size_t)tu.y * d.pred_stride[pl] + tu.x;
@@ -535,19 +468,106 @@ __global__ void __launch_bounds__(256) pack_levels_kernel(const int32_t *qcoeff,
     for (int i = lane; i < e; i += 32) o[i] = q[scan[i]];
 }
 
-static size_t tx_smem_bytes(int tx_size) {
-    const int w = h_txw[tx_size], h = h_txh[tx_size];
-    const int T = w > h ? w : h, bpc = TX_NT / T;
-    return (size_t)bpc * tx_pitch(w) * h * 4;
+// zero-out / re-pack of a 64-wide coefficient block, in place, with the energy of the dropped area
+__global__ void handle64_kernel(int32_t *io, int w, int h, unsigned long long *energy) {
+    extern __shared__ int32_t sm[];
+    const int kw = min(w, 32), kh = min(h, 32);
+    unsigned long long e = 0;
+    for (int i = threadIdx.x; i < w * h; i += blockDim.x) {
+        const int r = i / w, c = i - r * w;
+        const int32_t v = io[i];
+        sm[i] = v;
+        if (r >= kh || c >= kw) e += (unsigned long long)((long long)v * (long long)v);
+    }
+    __shared__ unsigned long long s_e;
+    if (threadIdx.x == 0) s_e = 0;
+    __syncthreads();
+    for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
+    if ((threadIdx.x & 31) == 0) atomicAdd(&s_e, e);
+    __syncthreads();
+    for (int i = threadIdx.x; i < w * h; i += blockDim.x) {
+        const int r = i / w, c = i - r * w;
+        io[i] = (kw != w && i < kw * kh) ? sm[(i / kw) * w + (i % kw)] : ((r >= kh || c >= kw) ? 0 : sm[i]);
+    }
+    if (threadIdx.x == 0) *energy = s_e;
 }
-static int tx_grid(int tx_size, int n) {
-    const int w = h_txw[tx_size], h = h_txh[tx_size];
-    const int T = w > h ? w : h, bpc = TX_NT / T;
-    return (n + bpc - 1) / bpc;
+
+// ---------------------------------------------------------------------------------------------------------------
+// Open-loop intra search of the TPL path, the flavour of presets >= 5 (tpl_opt_flag: DC_PRED only):
+// open_loop_intra_search_mb (EbMotionEstimation.c:3043-3155) for every 16x16 macroblock of a picture in one launch.
+// 16 threads per macroblock (one row / one column of the 16x16 DCT each), 8 macroblocks per CTA.  Neighbours come from
+// the source picture (update_neighbor_samples_array_open_loop_mb, EbEncIntraPrediction.c:1201: above = at most
+// min(32, width - x) samples of the row over the block, the rest 127; left = at most min(32, height - y) samples, the rest
+// 129), the predictor is dc_pred[x > 0][y > 0][TX_16X16], the cost svt_aom_satd of svt_av1_fwd_txfm2d_16x16(DCT_DCT) of the
+// residual.  Samples right of / below the picture are read as the replicated edge (the reference reads its padded input
+// picture there).
+// ---------------------------------------------------------------------------------------------------------------
+struct OisDev {
+    const uint8_t *y;
+    int stride, w, h, mbw, n_mb;
+    long long *cost;
+};
+__global__ void __launch_bounds__(TX_NT) ois_dc_kernel(const OisDev d) {
+    extern __shared__ int32_t sm[];
+    constexpr int W = 16, BPC = tx_bpc(W, W), pitch = tx_pitch(W);
+    const int lb = threadIdx.x / W, li = threadIdx.x % W;
+    const int mb = blockIdx.x * BPC + lb;
+    const bool live = mb < d.n_mb;
+    int32_t *buf = sm + lb * (pitch * W);
+    const TxCfg t = make_txcfg<2 /* TX_16X16 */>(2, 0 /* DCT_DCT */);
+    const int mx = live ? mb % d.mbw : 0, my = live ? mb / d.mbw : 0, x = mx * 16, y = my * 16;
+    // DC: lane li holds above[li] and left[li]; the 16 lanes of a macroblock are one half-warp
+    int a = 0, l = 0;
+    if (y > 0) a = li < min(32, d.w - x) ? d.y[(size_t)(y - 1) * d.stride + x + li] : 127;
+    if (x > 0) l = li < min(32, d.h - y) ? d.y[(size_t)(y + li) * d.stride + x - 1] : 129;
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) {
+        a += __shfl_xor_sync(0xffffffffu, a, o);
+        l += __shfl_xor_sync(0xffffffffu, l, o);
+    }
+    const int dc = (x > 0 && y > 0) ? (a + l + 16) >> 5 : y > 0 ? (a + 8) >> 4 : x > 0 ? (l + 8) >> 4 : 128;
+    if (live) {
+        const uint8_t *row = d.y + (size_t)min(y + li, d.h - 1) * d.stride;
+#pragma unroll
+        for (int c = 0; c < W; c++) buf[li * pitch + c] = (int)row[min(x + c, d.w - 1)] - dc;
+    }
+    __syncthreads();
+    fwd_txfm2d(buf, pitch, t, li, W, live);
+    long long s = 0; // lane li sums the row it transformed last
+    if (live)
+#pragma unroll
+        for (int c = 0; c < W; c++) s += abs(buf[li * pitch + c]);
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (live && li == 0) d.cost[mb] = s;
 }
-static void tx_attrs() {
+
+// ---------------------------------------------------------------------------------------------------------------
+// host helpers
+// ---------------------------------------------------------------------------------------------------------------
+static int coded_count(int tx_size) { return tx_coded(k_txw[tx_size]) * tx_coded(k_txh[tx_size]); }
+
+// Launch of n transform blocks of w x h: CTAs of TX_NT threads holding tx_bpc(w, h) blocks, each block in its own
+// odd-pitch int32 buffer in shared memory.
+struct TxLaunch {
+    int grid;
+    size_t smem;
+};
+static TxLaunch tx_launch(int w, int h, int n) {
+    const int bpc = tx_bpc(w, h);
+    return {(n + bpc - 1) / bpc, (size_t)bpc * tx_pitch(w) * h * sizeof(int32_t)};
+}
+
+// What every transform kernel needs on the current device, once per device: the constant tables and the kernels'
+// dynamic shared-memory limit.  Failures are fatal.
+static void tx_setup() {
     static PerDeviceOnce once;
     once.run([] {
+        txfm_upload_tables();
+        SVTB_CUDA_FATAL(cudaMemcpyToSymbol(c_txw, k_txw, sizeof(k_txw)));
+        SVTB_CUDA_FATAL(cudaMemcpyToSymbol(c_txh, k_txh, sizeof(k_txh)));
+        SVTB_CUDA_FATAL(cudaMemcpyToSymbol(c_vtx, k_vtx, sizeof(k_vtx)));
+        SVTB_CUDA_FATAL(cudaMemcpyToSymbol(c_htx, k_htx, sizeof(k_htx)));
         SVTB_ATTR(fwd_txfm_kernel, 64 * 1024);
         SVTB_ATTR(inv_txfm_kernel, 64 * 1024);
         SVTB_ATTR((encode_tu_kernel<uint8_t, -1>), 64 * 1024);
@@ -555,56 +575,66 @@ static void tx_attrs() {
     });
 }
 
+// dc/ac pairs; the quantize_fp family passes no zbin / quant_shift, which read as zeros
+static QuantTab quant_tab(const int16_t *zbin, const int16_t *round, const int16_t *quant, const int16_t *quant_shift,
+                          const int16_t *dequant) {
+    QuantTab q;
+    for (int i = 0; i < 2; i++) {
+        q.zbin[i] = zbin ? zbin[i] : 0;
+        q.round[i] = round[i];
+        q.quant[i] = quant[i];
+        q.quant_shift[i] = quant_shift ? quant_shift[i] : 0;
+        q.dequant[i] = dequant[i];
+    }
+    return q;
+}
+
+// plane pl (0 Y, 1 Cb, 2 Cr) of a frame and its stride in samples
+struct FramePlane {
+    void *ptr;
+    int stride;
+};
+static FramePlane frame_plane(const SvtB200Frame *f, int pl) {
+    return {pl == 0 ? f->y : pl == 1 ? f->cb : f->cr, pl == 0 ? f->stride_y : f->stride_c};
+}
+
 // ---- host side of the drop-ins --------------------------------------------------------------------------------
-static void fwd_dropin(int16_t *input, int32_t *output, uint32_t stride, int tx_type, int tx_size, int repack,
-                       uint64_t *energy_out, int pf_shift = 0) {
-    txfm_tables_init();
-    tx_attrs();
-    const int w = h_txw[tx_size], h = h_txh[tx_size];
-    Staging s({(size_t)w * h * 2, (size_t)w * h * 4, 8});
+static void fwd_dropin(int16_t *input, int32_t *output, uint32_t stride, int tx_type, int tx_size, int pf_shift) {
+    tx_setup();
+    const int w = k_txw[tx_size], h = k_txh[tx_size];
+    Staging s({(size_t)w * h * 2, (size_t)w * h * 4});
     SVTB_CUDA_FATAL(s.status());
     s.put_rows(0, input, stride, 2, w, h);
     SVTB_CUDA_FATAL(s.upload(0, 0));
     FwdArgs a;
     a.in = s.d<const int16_t>(0);
-    a.in_block_stride = 0;
-    a.in_stride = w;
     a.out = s.d<int32_t>(1);
-    a.tx_types = nullptr;
     a.tx_type = tx_type;
     a.tx_size = tx_size;
-    a.n_blocks = 1;
-    a.repack64 = repack;
     a.pf_shift = pf_shift;
-    a.energy = s.d<uint64_t>(2);
-    SVTB_LAUNCH(fwd_txfm_kernel, 1, TX_NT, tx_smem_bytes(tx_size), s.stream(), a);
-    SVTB_CUDA_FATAL(s.download(1, 2));
+    SVTB_LAUNCH(fwd_txfm_kernel, 1, TX_NT, tx_launch(w, h, 1).smem, s.stream(), a);
+    SVTB_CUDA_FATAL(s.download(1, 1));
     memcpy(output, s.h(1), (size_t)w * h * 4);
-    if (energy_out) memcpy(energy_out, s.h(2), 8);
 }
 
 static void inv_dropin(const int32_t *input, uint16_t *output_r, int32_t stride_r, uint16_t *output_w, int32_t stride_w,
                        int tx_type, int tx_size, int bd) {
-    txfm_tables_init();
-    tx_attrs();
-    const int w = h_txw[tx_size], h = h_txh[tx_size];
-    const int iw = w > 32 ? 32 : w, ih = h > 32 ? 32 : h;
-    Staging s({(size_t)iw * ih * 4, (size_t)w * h * 2, (size_t)w * h * 2});
+    tx_setup();
+    const int w = k_txw[tx_size], h = k_txh[tx_size];
+    const size_t nb = (size_t)coded_count(tx_size) * 4;
+    Staging s({nb, (size_t)w * h * 2, (size_t)w * h * 2});
     SVTB_CUDA_FATAL(s.status());
-    memcpy(s.h(0), input, (size_t)iw * ih * 4);
+    memcpy(s.h(0), input, nb);
     s.put_rows(1, output_r, stride_r, 2, w, h);
     SVTB_CUDA_FATAL(s.upload(0, 1));
     InvArgs a;
     a.in = s.d<const int32_t>(0);
     a.pred = s.d<const uint16_t>(1);
     a.recon = s.d<uint16_t>(2);
-    a.pred_block_stride = a.recon_block_stride = 0;
-    a.stride_r = a.stride_w = w;
     a.tx_type = tx_type;
     a.tx_size = tx_size;
-    a.n_blocks = 1;
     a.bd = bd;
-    SVTB_LAUNCH(inv_txfm_kernel, 1, TX_NT, tx_smem_bytes(tx_size), s.stream(), a);
+    SVTB_LAUNCH(inv_txfm_kernel, 1, TX_NT, tx_launch(w, h, 1).smem, s.stream(), a);
     SVTB_CUDA_FATAL(s.download(2, 2));
     s.get_rows(2, output_w, stride_w, 2, w, h);
 }
@@ -630,13 +660,7 @@ static void quant_dropin(int mode, const int32_t *coeff, intptr_t n, const int16
     a.qcoeff = s.d<int32_t>(4);
     a.dqcoeff = s.d<int32_t>(5);
     a.eob = s.d<uint16_t>(6);
-    for (int i = 0; i < 2; i++) {
-        a.q.zbin[i] = zbin ? zbin[i] : 0;
-        a.q.round[i] = round[i];
-        a.q.quant[i] = quant[i];
-        a.q.quant_shift[i] = quant_shift ? quant_shift[i] : 0;
-        a.q.dequant[i] = dequant[i];
-    }
+    a.q = quant_tab(zbin, round, quant, quant_shift, dequant);
     a.n = (int)n;
     a.log_scale = log_scale;
     a.mode = mode;
@@ -645,6 +669,106 @@ static void quant_dropin(int mode, const int32_t *coeff, intptr_t n, const int16
     memcpy(qcoeff, s.h(4), cb);
     memcpy(dqcoeff, s.h(5), cb);
     memcpy(eob, s.h(6), 2);
+}
+
+static void residual_dropin(const void *src, uint32_t ss, const void *pred, uint32_t ps, int16_t *res, uint32_t rs, uint32_t w,
+                            uint32_t h, int hbd) {
+    const size_t e = hbd ? 2 : 1, pb = (size_t)w * h * e;
+    Staging s({pb, pb, (size_t)w * h * 2});
+    SVTB_CUDA_FATAL(s.status());
+    s.put_rows(0, src, ss, e, w, h);
+    s.put_rows(1, pred, ps, e, w, h);
+    SVTB_CUDA_FATAL(s.upload(0, 1));
+    if (hbd)
+        SVTB_LAUNCH(residual_kernel<uint16_t>, 4, 256, 0, s.stream(), s.d<const uint16_t>(0), (int)w, s.d<const uint16_t>(1), (int)w,
+                    s.d<int16_t>(2), (int)w, (int)w, (int)h);
+    else
+        SVTB_LAUNCH(residual_kernel<uint8_t>, 4, 256, 0, s.stream(), s.d<const uint8_t>(0), (int)w, s.d<const uint8_t>(1), (int)w,
+                    s.d<int16_t>(2), (int)w, (int)w, (int)h);
+    SVTB_CUDA_FATAL(s.download(2, 2));
+    s.get_rows(2, res, rs, 2, w, h);
+}
+
+// ---- batched / picture-level entries ----------------------------------------------------------------------------
+// device-resident scan tables of one size, built on first use per device: [3][1024] inverse scans (raster position ->
+// scan index), then [3][1024] forward scans, each in scan_class order (default, row, column).  nullptr on a CUDA failure.
+const int16_t *scan_tables(int tx_size) {
+    static std::mutex mu;
+    static int16_t *tabs[64][19] = {};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev >= 64) return nullptr;
+    std::lock_guard<std::mutex> lk(mu);
+    if (tabs[dev][tx_size]) return tabs[dev][tx_size];
+    static int16_t hs[1024], hi[6][1024];
+    const int types[3] = {0, 10, 11}; // DCT_DCT (default scan), V_DCT (mrow), H_DCT (mcol)
+    const int n = coded_count(tx_size);
+    for (int k = 0; k < 3; k++) {
+        svt_b200_get_scan(tx_size, types[k], hs);
+        for (int i = 0; i < 1024; i++) hi[k][i] = hi[3 + k][i] = 0;
+        for (int i = 0; i < n; i++) {
+            hi[k][hs[i]] = (int16_t)i;
+            hi[3 + k][i] = hs[i];
+        }
+    }
+    int16_t *dp = nullptr;
+    if (cudaMalloc(&dp, sizeof(hi)) != cudaSuccess) return nullptr;
+    if (cudaMemcpy(dp, hi, sizeof(hi), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
+    tabs[dev][tx_size] = dp;
+    return dp;
+}
+
+template <int TS>
+void encode_kernel_launch(const EncodeDev &d, const TxLaunch &l, cudaStream_t st) {
+    if (d.hbd) SVTB_LAUNCH((encode_tu_kernel<uint16_t, TS>), l.grid, TX_NT, l.smem, st, d);
+    else SVTB_LAUNCH((encode_tu_kernel<uint8_t, TS>), l.grid, TX_NT, l.smem, st, d);
+}
+
+int encode_launch(const SvtB200EncodeParams *p, int pf_shape, const long long *qoff, const int32_t *out_idx,
+                  const SvtB200Frame *src, const SvtB200Frame *pred, const SvtB200Frame *recon, const SvtB200Tu *tus,
+                  int32_t n_tus, int32_t *qcoeff, uint16_t *eob, int32_t *cul_level, void *stream) {
+    if (!p || !src || !pred || !recon || !tus || !qcoeff || !eob || n_tus < 0 || p->tx_size < 0 || p->tx_size > 18 ||
+        src->bit_depth != pred->bit_depth || src->bit_depth != recon->bit_depth) {
+        set_error("svt_b200_encode_tus: bad argument");
+        return SVT_B200_ERR_ARG;
+    }
+    if (n_tus == 0) return SVT_B200_OK;
+    tx_setup();
+    static_assert(sizeof(SvtB200Tu) == sizeof(TuDev), "descriptor layout");
+    EncodeDev d;
+    for (int i = 0; i < 3; i++) {
+        const FramePlane s = frame_plane(src, i), pr = frame_plane(pred, i), rc = frame_plane(recon, i);
+        d.src[i] = s.ptr, d.src_stride[i] = s.stride;
+        d.pred[i] = pr.ptr, d.pred_stride[i] = pr.stride;
+        d.recon[i] = rc.ptr, d.recon_stride[i] = rc.stride;
+        const SvtB200QuantPlane &q = p->q[i];
+        d.q[i] = quant_tab(q.zbin, p->use_fp ? q.round_fp : q.round, p->use_fp ? q.quant_fp : q.quant, q.quant_shift, q.dequant);
+    }
+    d.bd = src->bit_depth;
+    d.hbd = src->bit_depth > 8;
+    d.tus = reinterpret_cast<const TuDev *>(tus);
+    d.n_tus = n_tus;
+    d.tx_size = p->tx_size;
+    d.quant_mode = p->use_fp ? 2 : 0;
+    d.qcoeff = qcoeff;
+    d.eob = eob;
+    d.cul_level = cul_level;
+    d.pf_shape = pf_shape;
+    d.qoff = qoff;
+    d.out_idx = out_idx;
+    const int16_t *tab = scan_tables(p->tx_size);
+    if (!tab) return SVT_B200_ERR_CUDA;
+    for (int i = 0; i < 3; i++) d.iscan[i] = tab + i * 1024;
+    cudaStream_t st = (cudaStream_t)stream;
+    const TxLaunch l = tx_launch(k_txw[p->tx_size], k_txh[p->tx_size], n_tus);
+    switch (p->tx_size) {
+    case 0: encode_kernel_launch<0>(d, l, st); break;
+    case 1: encode_kernel_launch<1>(d, l, st); break;
+    case 2: encode_kernel_launch<2>(d, l, st); break;
+    case 3: encode_kernel_launch<3>(d, l, st); break;
+    default: encode_kernel_launch<-1>(d, l, st); break;
+    }
+    SVTB_CUDA_TRY(cudaGetLastError());
+    return SVT_B200_OK;
 }
 
 } // namespace
@@ -656,17 +780,17 @@ extern "C" {
     void svt_av1_fwd_txfm2d_##W##x##H##_cuda(int16_t *input, int32_t *output, uint32_t input_stride, uint8_t tx_type, \
                                              uint8_t bit_depth) {                                                 \
         (void)bit_depth;                                                                                          \
-        fwd_dropin(input, output, input_stride, tx_type, TXS, 0, nullptr);                                        \
+        fwd_dropin(input, output, input_stride, tx_type, TXS, 0);                                                 \
     }                                                                                                             \
     void svt_av1_fwd_txfm2d_##W##x##H##_N2_cuda(int16_t *input, int32_t *output, uint32_t input_stride,           \
                                                 uint8_t tx_type, uint8_t bit_depth) {                             \
         (void)bit_depth;                                                                                          \
-        fwd_dropin(input, output, input_stride, tx_type, TXS, 0, nullptr, 1);                                     \
+        fwd_dropin(input, output, input_stride, tx_type, TXS, 1);                                                 \
     }                                                                                                             \
     void svt_av1_fwd_txfm2d_##W##x##H##_N4_cuda(int16_t *input, int32_t *output, uint32_t input_stride,           \
                                                 uint8_t tx_type, uint8_t bit_depth) {                             \
         (void)bit_depth;                                                                                          \
-        fwd_dropin(input, output, input_stride, tx_type, TXS, 0, nullptr, 2);                                     \
+        fwd_dropin(input, output, input_stride, tx_type, TXS, 2);                                                 \
     }
 FWD_DROPIN(4, 4, 0)
 FWD_DROPIN(8, 8, 1)
@@ -730,13 +854,20 @@ INV_RECT(16, 64, 17)
 INV_RECT(64, 16, 18)
 
 // svt_handle_transform64x64 & co. (aom_dsp_rtcd.h:222-245): operate in place on the w x h coefficient array
-#define HANDLE64(W, H, TXS)                                                                    \
-    uint64_t svt_handle_transform##W##x##H##_cuda(int32_t *output) {                           \
-        /* identity "transform" of the already transformed block is not available: run the */ \
-        /* zero-out / re-pack on the device through a plain copy kernel                      */ \
-        return svt_b200_handle_transform64(output, TXS);                                       \
-    }
-uint64_t svt_b200_handle_transform64(int32_t *output, int tx_size);
+uint64_t svt_b200_handle_transform64(int32_t *output, int tx_size) {
+    const int w = k_txw[tx_size], h = k_txh[tx_size];
+    const size_t nb = (size_t)w * h * 4;
+    Staging s({nb, 8});
+    SVTB_CUDA_FATAL(s.status());
+    memcpy(s.h(0), output, nb);
+    SVTB_CUDA_FATAL(s.upload(0, 0));
+    SVTB_LAUNCH(handle64_kernel, 1, 256, nb, s.stream(), s.d<int32_t>(0), w, h, s.d<unsigned long long>(1));
+    SVTB_CUDA_FATAL(s.download(0, 1));
+    memcpy(output, s.h(0), nb);
+    return *s.h<uint64_t>(1);
+}
+#define HANDLE64(W, H, TXS) \
+    uint64_t svt_handle_transform##W##x##H##_cuda(int32_t *output) { return svt_b200_handle_transform64(output, TXS); }
 HANDLE64(64, 64, 4)
 HANDLE64(32, 64, 11)
 HANDLE64(64, 32, 12)
@@ -780,23 +911,6 @@ void svt_av1_highbd_quantize_fp_cuda(const int32_t *coeff_ptr, intptr_t n_coeffs
                  eob_ptr, scan, nullptr, nullptr, log_scale);
 }
 
-static void residual_dropin(const void *src, uint32_t ss, const void *pred, uint32_t ps, int16_t *res, uint32_t rs, uint32_t w,
-                            uint32_t h, int hbd) {
-    const size_t e = hbd ? 2 : 1, pb = (size_t)w * h * e;
-    Staging s({pb, pb, (size_t)w * h * 2});
-    SVTB_CUDA_FATAL(s.status());
-    s.put_rows(0, src, ss, e, w, h);
-    s.put_rows(1, pred, ps, e, w, h);
-    SVTB_CUDA_FATAL(s.upload(0, 1));
-    if (hbd)
-        SVTB_LAUNCH(residual_kernel<uint16_t>, 4, 256, 0, s.stream(), s.d<const uint16_t>(0), (int)w, s.d<const uint16_t>(1), (int)w,
-                    s.d<int16_t>(2), (int)w, (int)w, (int)h);
-    else
-        SVTB_LAUNCH(residual_kernel<uint8_t>, 4, 256, 0, s.stream(), s.d<const uint8_t>(0), (int)w, s.d<const uint8_t>(1), (int)w,
-                    s.d<int16_t>(2), (int)w, (int)w, (int)h);
-    SVTB_CUDA_FATAL(s.download(2, 2));
-    s.get_rows(2, res, rs, 2, w, h);
-}
 void svt_residual_kernel8bit_cuda(uint8_t *input, uint32_t input_stride, uint8_t *pred, uint32_t pred_stride, int16_t *residual,
                                   uint32_t residual_stride, uint32_t area_width, uint32_t area_height) {
     residual_dropin(input, input_stride, pred, pred_stride, residual, residual_stride, area_width, area_height, 0);
@@ -805,51 +919,6 @@ void svt_residual_kernel16bit_cuda(uint16_t *input, uint32_t input_stride, uint1
                                    int16_t *residual, uint32_t residual_stride, uint32_t area_width, uint32_t area_height) {
     residual_dropin(input, input_stride, pred, pred_stride, residual, residual_stride, area_width, area_height, 1);
 }
-}
-
-// ---- zero-out / re-pack of 64-wide coefficient blocks on the device ----
-namespace {
-__global__ void handle64_kernel(int32_t *io, int w, int h, unsigned long long *energy) {
-    extern __shared__ int32_t sm[];
-    const int kw = min(w, 32), kh = min(h, 32);
-    unsigned long long e = 0;
-    for (int i = threadIdx.x; i < w * h; i += blockDim.x) {
-        const int r = i / w, c = i - r * w;
-        const int32_t v = io[i];
-        sm[i] = v;
-        if (r >= kh || c >= kw) e += (unsigned long long)((long long)v * (long long)v);
-    }
-    __shared__ unsigned long long s_e;
-    if (threadIdx.x == 0) s_e = 0;
-    __syncthreads();
-    for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(&s_e, e);
-    __syncthreads();
-    for (int i = threadIdx.x; i < w * h; i += blockDim.x) {
-        const int r = i / w, c = i - r * w;
-        io[i] = (kw != w && i < kw * kh) ? sm[(i / kw) * w + (i % kw)] : ((r >= kh || c >= kw) ? 0 : sm[i]);
-    }
-    if (threadIdx.x == 0) *energy = s_e;
-}
-} // namespace
-
-extern "C" uint64_t svt_b200_handle_transform64(int32_t *output, int tx_size) {
-    const int w = h_txw[tx_size], h = h_txh[tx_size];
-    const size_t nb = (size_t)w * h * 4;
-    Staging s({nb, 8});
-    SVTB_CUDA_FATAL(s.status());
-    memcpy(s.h(0), output, nb);
-    SVTB_CUDA_FATAL(s.upload(0, 0));
-    SVTB_LAUNCH(handle64_kernel, 1, 256, nb, s.stream(), s.d<int32_t>(0), w, h, s.d<unsigned long long>(1));
-    SVTB_CUDA_FATAL(s.download(0, 1));
-    memcpy(output, s.h(0), nb);
-    return *s.h<uint64_t>(1);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// batched / picture-level entries
-// ---------------------------------------------------------------------------------------------------------------
-extern "C" {
 
 // svt_av1_inv_txfm_add_c (EbInvTransforms.c:3302-3323): the low-bit-depth wrapper — widen the prediction to 16 bit, run
 // the (high-bit-depth) inverse transform at bd = 8, narrow the result.  TxfmParam (EbDefinitions.h:779-791) is read
@@ -868,7 +937,7 @@ void svt_av1_inv_txfm_add_cuda(const int32_t *dqcoeff, uint8_t *dst_r, int32_t s
         fprintf(stderr, "svt_av1_inv_txfm_add_cuda: tx_size %d / tx_type %d / lossless %d is not supported\n", tx_size, tx_type, tp->lossless);
         abort();
     }
-    const int w = h_txw[tx_size], h = h_txh[tx_size];
+    const int w = k_txw[tx_size], h = k_txh[tx_size];
     uint16_t tmp[64 * 64];
     for (int r = 0; r < h; r++)
         for (int c = 0; c < w; c++) tmp[r * 64 + c] = dst_r[(size_t)r * stride_r + c];
@@ -882,16 +951,11 @@ int svt_b200_get_scan(int tx_size, int tx_type, int16_t *scan_out) {
     // 2-D types: zig-zag (diagonals alternate for squares, fixed direction for rectangles); V_* (row-identity):
     // row scan; H_*: column scan; IDTX: default.
     if (tx_size < 0 || tx_size > 18 || tx_type < 0 || tx_type > 15 || !scan_out) return SVT_B200_ERR_ARG;
-    int w = h_txw[tx_size], h = h_txh[tx_size];
-    if (w > 32) w = 32;
-    if (h > 32) h = 32;
-    static const uint8_t vtx[16] = {0, 1, 0, 1, 2, 0, 2, 1, 2, 3, 0, 3, 1, 3, 2, 3};
-    static const uint8_t htx[16] = {0, 0, 1, 1, 0, 2, 2, 2, 1, 3, 3, 0, 3, 1, 3, 2};
-    const int vk = vtx[tx_type], hk = htx[tx_type];
+    const int w = tx_coded(k_txw[tx_size]), h = tx_coded(k_txh[tx_size]), cls = scan_class(k_vtx[tx_type], k_htx[tx_type]);
     int n = 0;
-    if (vk != 3 && hk == 3) { // V_DCT / V_ADST / V_FLIPADST: mrow_scan (raster)
+    if (cls == 1) { // V_DCT / V_ADST / V_FLIPADST: mrow_scan (raster)
         for (int i = 0; i < w * h; i++) scan_out[n++] = (int16_t)i;
-    } else if (vk == 3 && hk != 3) { // H_*: mcol_scan
+    } else if (cls == 2) { // H_*: mcol_scan
         for (int c = 0; c < w; c++)
             for (int r = 0; r < h; r++) scan_out[n++] = (int16_t)(r * w + c);
     } else {
@@ -916,12 +980,6 @@ int svt_b200_get_scan(int tx_size, int tx_type, int16_t *scan_out) {
     return n;
 }
 
-
-} // extern "C"
-namespace {
-const int16_t *scan_tables(int tx_size);
-}
-extern "C" {
 // see include/svt_av1_b200.h
 int svt_b200_pack_levels(int32_t tx_size, int32_t tx_class, const int32_t *qcoeff, const uint16_t *eob, int32_t n_tus, int32_t *packed,
                          uint32_t *offsets, uint32_t *total, void *stream) {
@@ -948,42 +1006,12 @@ int svt_b200_pack_levels_at(int32_t tx_size, int32_t tx_class, const int32_t *qc
     }
     const int16_t *tab = scan_tables(tx_size);
     if (!tab) return SVT_B200_ERR_CUDA;
-    const int n = (h_txw[tx_size] > 32 ? 32 : h_txw[tx_size]) * (h_txh[tx_size] > 32 ? 32 : h_txh[tx_size]);
+    const int n = coded_count(tx_size);
     SVTB_LAUNCH(eob_scan_kernel, 1, 1024, 0, st, eob, n_tus, offsets, total, base);
     SVTB_LAUNCH(pack_levels_kernel, (n_tus + 7) / 8, 256, 0, st, qcoeff, eob, offsets, tab + 3072 + tx_class * 1024, n_tus, n, packed);
     SVTB_CUDA_TRY(cudaGetLastError());
     return SVT_B200_OK;
 }
-
-} // extern "C"
-namespace {
-// device-resident inverse scan tables: [device][tx_size] -> 3 x 1024 int16
-const int16_t *scan_tables(int tx_size) { // [3][1024] inverse scans, then [3][1024] forward scans
-    static std::mutex mu;
-    static int16_t *tabs[64][19] = {};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev >= 64) return nullptr;
-    std::lock_guard<std::mutex> lk(mu);
-    if (tabs[dev][tx_size]) return tabs[dev][tx_size];
-    static int16_t hs[1024], hi[6][1024];
-    const int types[3] = {0, 10, 11}; // DCT_DCT (default scan), V_DCT (mrow), H_DCT (mcol)
-    const int n = (h_txw[tx_size] > 32 ? 32 : h_txw[tx_size]) * (h_txh[tx_size] > 32 ? 32 : h_txh[tx_size]);
-    for (int k = 0; k < 3; k++) {
-        svt_b200_get_scan(tx_size, types[k], hs);
-        for (int i = 0; i < 1024; i++) hi[k][i] = hi[3 + k][i] = 0;
-        for (int i = 0; i < n; i++) {
-            hi[k][hs[i]] = (int16_t)i;
-            hi[3 + k][i] = hs[i];
-        }
-    }
-    int16_t *dp = nullptr;
-    if (cudaMalloc(&dp, sizeof(hi)) != cudaSuccess) return nullptr;
-    if (cudaMemcpy(dp, hi, sizeof(hi), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
-    tabs[dev][tx_size] = dp;
-    return dp;
-}
-} // namespace
-extern "C" {
 
 int svt_b200_encode_tus(const SvtB200EncodeParams *p, const SvtB200Frame *src, const SvtB200Frame *pred,
                         const SvtB200Frame *recon, const SvtB200Tu *tus, int32_t n_tus, int32_t *qcoeff, uint16_t *eob,
@@ -992,82 +1020,10 @@ int svt_b200_encode_tus(const SvtB200EncodeParams *p, const SvtB200Frame *src, c
     return svt_b200_encode_tus_cul(p, src, pred, recon, tus, n_tus, qcoeff, eob, nullptr, stream);
 }
 
-static int encode_launch(const SvtB200EncodeParams *p, int pf_shape, const long long *qoff, const int32_t *out_idx,
-                         const SvtB200Frame *src, const SvtB200Frame *pred, const SvtB200Frame *recon, const SvtB200Tu *tus,
-                         int32_t n_tus, int32_t *qcoeff, uint16_t *eob, int32_t *cul_level, void *stream);
-
 int svt_b200_encode_tus_cul(const SvtB200EncodeParams *p, const SvtB200Frame *src, const SvtB200Frame *pred,
                             const SvtB200Frame *recon, const SvtB200Tu *tus, int32_t n_tus, int32_t *qcoeff, uint16_t *eob,
                             int32_t *cul_level, void *stream) {
     return encode_launch(p, 0, nullptr, nullptr, src, pred, recon, tus, n_tus, qcoeff, eob, cul_level, stream);
-}
-
-static int encode_launch(const SvtB200EncodeParams *p, int pf_shape, const long long *qoff, const int32_t *out_idx,
-                         const SvtB200Frame *src, const SvtB200Frame *pred, const SvtB200Frame *recon, const SvtB200Tu *tus,
-                         int32_t n_tus, int32_t *qcoeff, uint16_t *eob, int32_t *cul_level, void *stream) {
-    if (!p || !src || !pred || !recon || !tus || !qcoeff || !eob || n_tus < 0 || p->tx_size < 0 || p->tx_size > 18 ||
-        src->bit_depth != pred->bit_depth || src->bit_depth != recon->bit_depth) {
-        set_error("svt_b200_encode_tus: bad argument");
-        return SVT_B200_ERR_ARG;
-    }
-    if (n_tus == 0) return SVT_B200_OK;
-    txfm_tables_init();
-    tx_attrs();
-    static_assert(sizeof(SvtB200Tu) == sizeof(TuDev), "descriptor layout");
-    EncodeDev d;
-    const SvtB200Frame *fr[3] = {src, pred, recon};
-    for (int i = 0; i < 3; i++) {
-        d.src[i] = i == 0 ? fr[0]->y : i == 1 ? fr[0]->cb : fr[0]->cr;
-        d.pred[i] = i == 0 ? fr[1]->y : i == 1 ? fr[1]->cb : fr[1]->cr;
-        d.recon[i] = i == 0 ? fr[2]->y : i == 1 ? fr[2]->cb : fr[2]->cr;
-        d.src_stride[i] = i == 0 ? fr[0]->stride_y : fr[0]->stride_c;
-        d.pred_stride[i] = i == 0 ? fr[1]->stride_y : fr[1]->stride_c;
-        d.recon_stride[i] = i == 0 ? fr[2]->stride_y : fr[2]->stride_c;
-        for (int k = 0; k < 2; k++) {
-            d.q[i].zbin[k] = p->q[i].zbin[k];
-            d.q[i].round[k] = p->use_fp ? p->q[i].round_fp[k] : p->q[i].round[k];
-            d.q[i].quant[k] = p->use_fp ? p->q[i].quant_fp[k] : p->q[i].quant[k];
-            d.q[i].quant_shift[k] = p->q[i].quant_shift[k];
-            d.q[i].dequant[k] = p->q[i].dequant[k];
-        }
-    }
-    d.bd = src->bit_depth;
-    d.hbd = src->bit_depth > 8;
-    d.tus = reinterpret_cast<const TuDev *>(tus);
-    d.n_tus = n_tus;
-    d.tx_size = p->tx_size;
-    d.quant_mode = p->use_fp ? 2 : 0;
-    d.qcoeff = qcoeff;
-    d.eob = eob;
-    d.cul_level = cul_level;
-    d.pf_shape = pf_shape;
-    d.qoff = qoff;
-    d.out_idx = out_idx;
-    // inverse scan tables of this size: built once per (device, tx_size) and kept resident (`scratch` is unused since
-    // then; the parameter stays for ABI stability)
-    const int16_t *tab = scan_tables(p->tx_size);
-    if (!tab) return SVT_B200_ERR_CUDA;
-    for (int i = 0; i < 3; i++) d.iscan[i] = tab + i * 1024;
-    cudaStream_t st = (cudaStream_t)stream;
-    const int grid = tx_grid(p->tx_size, n_tus);
-    const size_t smem = tx_smem_bytes(p->tx_size);
-#define SVTB_ENC(TSV)                                                                          \
-    do {                                                                                       \
-        if (d.hbd)                                                                             \
-            SVTB_LAUNCH((encode_tu_kernel<uint16_t, TSV>), grid, TX_NT, smem, st, d);          \
-        else                                                                                   \
-            SVTB_LAUNCH((encode_tu_kernel<uint8_t, TSV>), grid, TX_NT, smem, st, d);           \
-    } while (0)
-    switch (p->tx_size) {
-    case 0: SVTB_ENC(0); break;
-    case 1: SVTB_ENC(1); break;
-    case 2: SVTB_ENC(2); break;
-    case 3: SVTB_ENC(3); break;
-    default: SVTB_ENC(-1); break;
-    }
-#undef SVTB_ENC
-    SVTB_CUDA_TRY(cudaGetLastError());
-    return SVT_B200_OK;
 }
 
 // av1_estimate_transform's dispatcher generality for the fused path (VERDICT r1 a11): a HOST list of transform units of MIXED
@@ -1097,7 +1053,7 @@ int svt_b200_encode_tus_ex(const SvtB200EncodeParamsEx *p, const SvtB200Frame *s
             return SVT_B200_ERR_ARG;
         }
         qcoeff_offsets[i] = off;
-        off += (long long)std::min<int>(h_txw[t.tx_size], 32) * std::min<int>(h_txh[t.tx_size], 32);
+        off += coded_count(t.tx_size);
     }
     qcoeff_offsets[n_tus] = off;
     if (n_tus == 0) return SVT_B200_OK;
@@ -1142,71 +1098,6 @@ int svt_b200_encode_tus_ex(const SvtB200EncodeParamsEx *p, const SvtB200Frame *s
     SVTB_CUDA_TRY(cudaStreamSynchronize(st));
     return rc;
 }
-} // extern "C"
-
-// ---------------------------------------------------------------------------------------------------------------
-// Open-loop intra search of the TPL path, the flavour of presets >= 5 (tpl_opt_flag: DC_PRED only):
-// open_loop_intra_search_mb (EbMotionEstimation.c:3043-3155) for every 16x16 macroblock of a picture in one launch.
-// 16 threads per macroblock (one row / one column of the 16x16 DCT each), 8 macroblocks per CTA.  Neighbours come from
-// the source picture (update_neighbor_samples_array_open_loop_mb, EbEncIntraPrediction.c:1201: above = at most
-// min(32, width - x) samples of the row over the block, the rest 127; left = at most min(32, height - y) samples, the rest
-// 129), the predictor is dc_pred[x > 0][y > 0][TX_16X16], the cost svt_aom_satd of svt_av1_fwd_txfm2d_16x16(DCT_DCT) of the
-// residual.  Samples right of / below the picture are read as the replicated edge (the reference reads its padded input
-// picture there).
-// ---------------------------------------------------------------------------------------------------------------
-namespace {
-struct OisDev {
-    const uint8_t *y;
-    int stride, w, h, mbw, n_mb;
-    long long *cost;
-};
-__global__ void __launch_bounds__(TX_NT) ois_dc_kernel(const OisDev d) {
-    extern __shared__ int32_t sm[];
-    constexpr int W = 16, T = 16, BPC = TX_NT / T;
-    const int pitch = tx_pitch(W);
-    const int lb = threadIdx.x / T, li = threadIdx.x % T;
-    const int mb = blockIdx.x * BPC + lb;
-    const bool live = mb < d.n_mb;
-    int32_t *buf = sm + lb * (pitch * W);
-    const TxCfg t = make_txcfg(2 /* TX_16X16 */, 0 /* DCT_DCT */);
-    const int mx = live ? mb % d.mbw : 0, my = live ? mb / d.mbw : 0, x = mx * 16, y = my * 16;
-    // DC: lane li holds above[li] and left[li]; the 16 lanes of a macroblock are one half-warp
-    int a = 0, l = 0;
-    if (y > 0) a = li < min(32, d.w - x) ? d.y[(size_t)(y - 1) * d.stride + x + li] : 127;
-    if (x > 0) l = li < min(32, d.h - y) ? d.y[(size_t)(y + li) * d.stride + x - 1] : 129;
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) {
-        a += __shfl_xor_sync(0xffffffffu, a, o);
-        l += __shfl_xor_sync(0xffffffffu, l, o);
-    }
-    const int dc = (x > 0 && y > 0) ? (a + l + 16) >> 5 : y > 0 ? (a + 8) >> 4 : x > 0 ? (l + 8) >> 4 : 128;
-    if (live) {
-        const uint8_t *row = d.y + (size_t)min(y + li, d.h - 1) * d.stride;
-#pragma unroll
-        for (int c = 0; c < W; c++) buf[li * pitch + c] = (int)row[min(x + c, d.w - 1)] - dc;
-    }
-    __syncthreads();
-    if (live) {
-        const int fs0 = t.fs0, fs1 = t.fs1;
-        fwd_1d_pass(buf + li, pitch, t.h, t.vk, t.cbc, [=](int32_t v) { return (int32_t)((uint32_t)v << fs0); },
-                    [=](int32_t v) { return fs1 ? round_shift64((long long)v, -fs1) : v; });
-    }
-    __syncthreads();
-    long long s = 0;
-    if (live) {
-        const int fs2 = t.fs2;
-        fwd_1d_pass(buf + li * pitch, 1, t.w, t.hk, t.cbr, [](int32_t v) { return v; },
-                    [=](int32_t v) { return fs2 ? round_shift64((long long)v, -fs2) : v; });
-#pragma unroll
-        for (int c = 0; c < W; c++) s += abs(buf[li * pitch + c]);
-    }
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (live && li == 0) d.cost[mb] = s;
-}
-} // namespace
-
-extern "C" {
 
 // pic: 8-bit picture (the luma plane is read); cost: DEVICE int64 [mb rows][mb cols], mb cols = (width + 15) / 16 =
 // the reference's mb_stride; every entry is OisMbResults::intra_cost of that macroblock, its intra_mode is DC_PRED.
@@ -1215,14 +1106,14 @@ int svt_b200_ois_dc_picture(const SvtB200Frame *pic, int64_t *cost, void *stream
         set_error("svt_b200_ois_dc_picture: bad argument (8-bit pictures)");
         return SVT_B200_ERR_ARG;
     }
-    txfm_tables_init();
+    tx_setup();
     OisDev d;
     d.y = (const uint8_t *)pic->y, d.stride = pic->stride_y, d.w = pic->width, d.h = pic->height;
     d.mbw = (pic->width + 15) / 16;
     d.n_mb = d.mbw * ((pic->height + 15) / 16);
     d.cost = (long long *)cost;
-    const int bpc = TX_NT / 16;
-    SVTB_LAUNCH(ois_dc_kernel, (d.n_mb + bpc - 1) / bpc, TX_NT, (size_t)bpc * tx_pitch(16) * 16 * sizeof(int32_t), (cudaStream_t)stream, d);
+    const TxLaunch l = tx_launch(16, 16, d.n_mb);
+    SVTB_LAUNCH(ois_dc_kernel, l.grid, TX_NT, l.smem, (cudaStream_t)stream, d);
     SVTB_CUDA_TRY(cudaGetLastError());
     return SVT_B200_OK;
 }

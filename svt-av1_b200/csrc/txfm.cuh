@@ -10,25 +10,18 @@
 #pragma once
 #include <cmath>
 #include <cstdint>
-#include <mutex>
 
 #include "common.cuh"
 
 namespace svtb200 {
 
-// per-translation-unit copies (no relocatable device code): every .cu that includes this header calls
-// txfm_tables_init() before launching a kernel that uses them
+// per-translation-unit copies (no relocatable device code): every .cu that includes this header uploads them with
+// txfm_upload_tables() once per device before launching a kernel that uses them
 static __constant__ int32_t c_cospi[4][64]; // cos_bit 10..13
 static __constant__ int32_t c_sinpi[4][5];
 
-// host: fills the constant tables on the current device (idempotent per device)
-static void txfm_tables_init() {
-    static std::mutex mu;
-    static bool done[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    std::lock_guard<std::mutex> lk(mu);
-    if (dev < 64 && done[dev]) return;
+// host: fills the constant tables on the current device
+static void txfm_upload_tables() {
     int32_t cospi[4][64];
     // eb_av1_cospi_arr_data: round(cos(i*pi/128) * 2^bit).  eb_av1_sinpi_arr_data is hand-adjusted in the reference
     // (sinpi[1] + sinpi[2] == sinpi[4]) and therefore kept as data.
@@ -38,7 +31,6 @@ static void txfm_tables_init() {
         for (int i = 0; i < 64; i++) cospi[b - 10][i] = (int32_t)floor(cos(M_PI * i / 128.0) * (double)(1 << b) + 0.5);
     SVTB_CUDA_FATAL(cudaMemcpyToSymbol(c_cospi, cospi, sizeof(cospi)));
     SVTB_CUDA_FATAL(cudaMemcpyToSymbol(c_sinpi, sinpi, sizeof(sinpi)));
-    if (dev < 64) done[dev] = true;
 }
 
 // Common/Codec/EbInvTransforms.h:285-312: 32-bit wrapping products, 64-bit sum, rounding shift
@@ -522,5 +514,56 @@ struct TxCfg {
     int rect; // |log2(w/h)| == 1
 };
 
+// ---- 2-D transforms in place on a block in shared memory (w x h int32, row pitch `pitch`) -------------------
+// Lane li of the block's T lanes takes the columns and the rows li, li + T, ...  Each body holds the barrier between
+// its two passes, so every thread of the CTA calls it; `live` keeps the lanes of a missing block out of the passes.
+// The size comes from t: where make_txcfg<TS> fixed it at compile time, the loop bounds and the 1-D sizes fold.
+
+// av1_transform_two_d_* without the input flips (the caller applies them as it loads the block): the column pass
+// with shifts 0 and 1, then the row pass with shift 2 and the 1/sqrt(2) scaling of 2:1 rectangles.
+__device__ __forceinline__ void fwd_txfm2d(int32_t *buf, int pitch, const TxCfg &t, int li, int T, bool live) {
+    if (live)
+        for (int c = li; c < t.w; c += T) {
+            const int fs0 = t.fs0, fs1 = t.fs1;
+            fwd_1d_pass(buf + c, pitch, t.h, t.vk, t.cbc, [=](int32_t v) { return (int32_t)((uint32_t)v << fs0); },
+                        [=](int32_t v) { return fs1 ? round_shift64((long long)v, -fs1) : v; });
+        }
+    __syncthreads();
+    if (live)
+        for (int r = li; r < t.h; r += T) {
+            const int fs2 = t.fs2, rect = t.rect;
+            fwd_1d_pass(buf + r * pitch, 1, t.w, t.hk, t.cbr, [](int32_t v) { return v; }, [=](int32_t v) {
+                if (fs2) v = round_shift64((long long)v, -fs2);
+                if (rect) v = round_shift64((long long)v * 5793, 12);
+                return v;
+            });
+        }
+}
+
+// svt_av1_inv_txfm2d_add_* without the output flips and the prediction add (the caller's store): the row pass with
+// the rectangular scaling and shift 0, then the column pass with shift 1; bd sets the reference's clamps.  A live lane
+// runs first() before its rows: the fused kernel publishes a unit's eob there, inside the same live branch.
+template <typename First>
+__device__ __forceinline__ void inv_txfm2d(int32_t *buf, int pitch, const TxCfg &t, int bd, int li, int T, bool live, First first) {
+    const int range_row = bd == 8 ? 16 : bd == 10 ? 18 : 20, range_col = bd == 8 ? 16 : bd == 10 ? 16 : 18;
+    if (live) {
+        first();
+        for (int r = li; r < t.h; r += T) {
+            const int rect = t.rect, is0 = t.is0;
+            inv_1d_pass(buf + r * pitch, 1, t.w, t.hk, 12, range_row, [=](int32_t v) {
+                if (rect) v = round_shift64((long long)v * 2896, 12);
+                return clampv(v, bd + 8);
+            }, [=](int32_t v) { return is0 ? round_shift64((long long)v, -is0) : v; });
+        }
+    }
+    __syncthreads();
+    if (live) {
+        const int col_clamp = max(bd + 6, 16);
+        for (int c = li; c < t.w; c += T) {
+            inv_1d_pass(buf + c, pitch, t.h, t.vk, 12, range_col, [=](int32_t v) { return clampv(v, col_clamp); },
+                        [](int32_t v) { return round_shift64((long long)v, 4); });
+        }
+    }
+}
 
 } // namespace svtb200
